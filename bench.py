@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """bench.py -- the headline benchmark (BASELINE.json: uncompressed GB/s, level-3 compress + decompress).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--chunks C] [--level L]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--chunks C] [--level L] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 A *step* is one pass of the hot path over one batch: every rank compresses its shard of C 128 KB chunks
 (level 3, one frame per chunk, sizes scanned and frames concatenated on the device) and decompresses the
 resulting stream back.  Default workload = BASELINE.json configs[1]: a 1 GiB synthetic Silesia-mix corpus
-(8192 x 131072 B, seed 20240901) on one B200.  With N GPUs every rank gets its own 8192-chunk shard (weak
+(8192 x 131072 B, seed 20240901) on one H100.  With N GPUs every rank gets its own 8192-chunk shard (weak
 scaling); frames are independent so there is no data-path exchange, only an all_gather of the per-frame sizes
 (the global stream index) and the timing reduction.
 
@@ -136,7 +136,7 @@ def cpu_model() -> str:
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampled every 200 ms while the timed region runs (B200_PROFILING.md)."""
+    """nvidia-smi sampled every 200 ms while the timed region runs: SM clock and the reasons it was held down."""
 
     def __init__(self, index: int):
         self.samples = []
@@ -144,7 +144,7 @@ class ClockSampler:
         self.index = index
 
     def start(self):
-        q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+        q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), f"--query-gpu={q}", "--format=csv,noheader,nounits", "-lms", "200"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -158,12 +158,14 @@ class ClockSampler:
 
     def stop(self):
         if self.proc:
-            self.proc.terminate()
+            self.proc.terminate(); self.proc.wait()
         sm = [float(s[0]) for s in self.samples if s and s[0].replace(".", "").isdigit()]
         mx = [float(s[1]) for s in self.samples if len(s) > 1 and s[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = sorted({names[k] for s in self.samples if len(s) >= 7 for k in range(4) if s[3 + k].lower().startswith("active")})
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons, "samples": len(sm)}
+        lim = [float(s[7]) for s in self.samples if len(s) > 7 and s[7].replace(".", "").isdigit()]
+        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "power_limit_w": max(lim) if lim else None,
+                "reasons": reasons, "samples": len(sm)}
 
 
 # ----------------------------------------------------------------------------- main
@@ -179,12 +181,15 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the sub-records (levels, configs[3], configs[4])")
     ap.add_argument("--strong", action="store_true", help="also run the strong-scaling data-plane record at N = 1")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last one computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be at least 1 and --warmup at least 0")
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
     from zstd_jni_b200 import corpus
 
     config = {"workload": f"{args.chunks} x {CHUNK} B synthetic Silesia-mix chunks per GPU (seed {corpus.SEED}), level {args.level}, one frame per chunk",
-              "chunks_per_gpu": args.chunks, "chunk_bytes": CHUNK, "level": args.level, "cache": "inputs_larger_than_L2 (1 GiB working set per pass vs 126 MB L2)",
+              "chunks_per_gpu": args.chunks, "chunk_bytes": CHUNK, "level": args.level, "cache": "inputs_larger_than_L2 (1 GiB working set per pass vs 50 MB L2)",
               "parallelism": f"frames sharded over {args.gpus} GPU(s), no data-path collective"}
 
     if args.impl == "reference":
@@ -278,8 +283,6 @@ def main():
         for _ in range(args.warmup):
             step()
         barrier()
-        assert torch.equal(d_back, d_src) and bool((d_res == CHUNK).all()), "device round trip mismatch"
-        csize = int(d_sizes.sum().item())
         sampler = ClockSampler(local); sampler.start()
         launches0 = ctx.kernelLaunches()
         ctx.setOption("timing", 1)          # the library brackets every kernel with CUDA events on its launching stream
@@ -295,6 +298,10 @@ def main():
         launches = ctx.kernelLaunches() - launches0
         ktimes = ctx.kernelTimes()
         clocks = sampler.stop()
+        assert torch.equal(d_back, d_src) and bool((d_res == CHUNK).all()), "device round trip mismatch"
+        csize = int(d_sizes.sum().item())
+        if args.dump_outputs and rank == 0:
+            dump_outputs(Path(args.dump_outputs), n, d_sizes, d_ooff, d_out, d_back, d_res)
         # The entropy stage runs beside the parse (one timed entry, "k_parse+k_entropy"); a short pass with the two serialized gives the
         # stage times on their own -- reported as such, not part of the timed region.
         ctx.setOption("entropy_overlap", 0)
@@ -337,11 +344,13 @@ def main():
         de(K - 1)
         torch.cuda.synchronize()
     e2e_run(2); barrier()
-    e2e_steps = max(4, min(args.steps, 32))          # the pipeline fills and drains once per run (~60 ms that no step can hide): the K steps asked for, at least 4
+    for b in h_back:
+        b.zero_()          # the check below must see only what the timed run wrote
+    e2e_steps = args.steps          # the pipeline fills and drains once per run, a cost no step can hide: few steps understate the rate
     t0 = time.perf_counter()
     e2e_run(e2e_steps)
     e2e_s = (time.perf_counter() - t0) / e2e_steps
-    assert torch.equal(h_back[(e2e_steps - 1) % 2], h_src) and torch.equal(h_back[e2e_steps % 2], h_src), "e2e round trip mismatch"
+    assert all(torch.equal(h_back[k % 2], h_src) for k in range(min(e2e_steps, 2))), "e2e round trip mismatch"
     te = torch.tensor([e2e_s], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(te, op=dist.ReduceOp.MAX)
@@ -362,7 +371,7 @@ def main():
     if peaks_path.exists():
         peak = float(json.loads(peaks_path.read_text())["hbm_gbs"]); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak = 6650.0; peak_src = "fallback (B200_PROFILING.md 6.65 TB/s)"
+        peak = 3350.0; peak_src = "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
     algo_bytes = U + csize                                  # SURVEY.md 8(d): uncompressed + compressed bytes of every frame in the launch
     # per-kernel averages over the timed region (rank 0), from the events the library records around every launch
     kernels = {k: v[0] for k, v in ktimes.items()}
@@ -371,22 +380,14 @@ def main():
     phases = {"compress": k_comp, "scan+compact": k_pack, "decompress": k_dec}          # API-call brackets, max over ranks
     payload = {k: v for k, v in kernels.items() if k not in ("k_order", "k_parse(estimate)", "k_dec_prepare", "k_decompress")}
     dom = max(payload, key=payload.get)
-    traffic = {}
-    tpath = ROOT / "profiles" / "dram_traffic.json"          # dram__bytes_read.sum + dram__bytes_write.sum per launch (ncu --set full)
-    if tpath.exists():
-        tj = json.loads(tpath.read_text())
-        if tj.get("chunks_per_gpu") == n and tj.get("level") == args.level:
-            traffic = tj.get("kernels", {})
     # algorithmic bytes per kernel (payload kernels only): what the stage has to read and write once, SURVEY.md 8(d) split by stage
     stage_bytes = {PAIR: (U + csize, "the two compression stages, overlapped: the input is read, the frames are written"),
                    "k_parse": (U, "reads the input"), "k_entropy": (U + csize, "reads the input (literals), writes the frames"),
                    "k_scan_sizes+k_compact": (2 * csize, "reads and writes the frames"), "k_dec_chains": (csize, "reads the frames' bitstreams"),
                    "k_dec_exec": (U, "writes the regenerated bytes")}
-    if PAIR in kernels and "k_parse" in traffic and "k_entropy" in traffic:
-        traffic = dict(traffic); traffic[PAIR] = traffic["k_parse"] + traffic["k_entropy"]
     def roof(name, nbytes, table=None):
         a = nbytes / ((table or kernels)[name] * 1e-3) / 1e9
-        return {"bound": "hbm", "achieved": a, "peak": peak, "unit": "GB/s", "frac": a / peak, "traffic": traffic.get(name), "bytes": nbytes}
+        return {"bound": "hbm", "achieved": a, "peak": peak, "unit": "GB/s", "frac": a / peak, "bytes": nbytes}
     roofline_all = {k: dict(roof(k, stage_bytes[k][0]), what=stage_bytes[k][1], timed="timed region") for k in kernels if k in stage_bytes}
     for k in ("k_parse", "k_entropy"):
         if k in serial and k not in roofline_all:
@@ -403,7 +404,7 @@ def main():
                    "api": "zstdb200_compress_chunks_begin/_end + zstdb200_decompress_frames_begin/_end on 4 work sets, pinned host buffers; "
                           "every step's input goes H2D and its result D2H inside the timed region, steps overlap",
                    "steps": e2e_steps, "synchronous_ms_per_step": sync_s * 1e3, "numa": numa},
-           "gpu_launches": int(launches), "clocks": clocks}
+           "gpu_launches": int(launches), "gpu": torch.cuda.get_device_name(dev), "clocks": clocks}
     if strong is not None:
         out["strong"] = strong
     if not args.no_cpu_baseline and world == 1:
@@ -433,6 +434,29 @@ def main():
     print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()
+
+
+# ----------------------------------------------------------------------------- output dump
+DUMP_FRAMES = 32          # whole chunks written out: 32 x 128 KB regenerated bytes plus their frames, under 34 MB as float32
+DUMP_SEED = 20241015
+
+
+def dump_outputs(out_dir: Path, n, d_sizes, d_ooff, d_out, d_back, d_res):
+    """What the device-resident path hands its caller after the last timed step, as float arrays: every frame's compressed size
+    and offset in the packed stream, every chunk's decompression result, and the bytes of a fixed, seeded sample of frames (the
+    packed frames and the chunks regenerated from them).  The inputs are seeded too, so two builds run with the same arguments
+    can be compared array for array."""
+    import torch
+    out_dir.mkdir(parents=True, exist_ok=True)
+    pick = np.sort(np.random.default_rng(DUMP_SEED).choice(n, size=min(DUMP_FRAMES, n), replace=False))
+    sizes = d_sizes.cpu().numpy(); offs = d_ooff.cpu().numpy()
+    frames = np.concatenate([d_out[int(offs[i]):int(offs[i]) + int(sizes[i])].cpu().numpy() for i in pick])
+    chunks = d_back.view(n, CHUNK)[torch.from_numpy(pick).to(d_back.device)].cpu().numpy()
+    arrays = {"frame_sizes": sizes.astype(np.float64), "frame_offsets": offs.astype(np.float64),
+              "decompressed_sizes": d_res.cpu().numpy().astype(np.float64), "sample_index": pick.astype(np.float64),
+              "sample_frames": frames.astype(np.float32), "sample_chunks": chunks.astype(np.float32)}
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a)
 
 
 # ----------------------------------------------------------------------------- sub-records

@@ -1,5 +1,5 @@
 /*
- * zstdb200.h -- C ABI of the B200-native Zstandard block codec (libzstdb200.so).
+ * zstdb200.h -- C ABI of the GPU-native (H100) Zstandard block codec (libzstdb200.so).
  *
  * Two layers are exported, both plain C (pointers + sizes, no torch / C++ types):
  *

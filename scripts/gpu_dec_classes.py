@@ -1,4 +1,4 @@
-"""Decoder latency per corpus class: 148 frames of ONE class (about one warp per SM), then 4736 of it."""
+"""Decoder latency per corpus class: one frame of ONE class per SM, then 32 per SM."""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -8,10 +8,11 @@ from zstd_jni_b200.zstd import ZstdBatchContext
 L = _native.lib()
 ctx = ZstdBatchContext(0); ctx.setOption("timing", 1)
 dev = torch.device("cuda:0")
+sms = torch.cuda.get_device_properties(dev).multi_processor_count
 stride = (L.ZSTD_compressBound(131072) + 32 + 63) // 64 * 64
 buf = C.create_string_buffer(4096)
 stream = torch.cuda.Stream(); st = stream.cuda_stream
-counts = [int(a) for a in sys.argv[1:]] or [148, 4736]
+counts = [int(a) for a in sys.argv[1:]] or [sms, 32 * sms]
 for cls in range(8):
     for n in counts:
         data = np.stack([corpus.chunk(cls + 8 * (i % 64)) for i in range(n)])

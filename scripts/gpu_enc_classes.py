@@ -1,4 +1,4 @@
-"""k_parse latency of a lone warp per corpus class: 148 frames of ONE class (one warp per SM), then 4736 of it (a full wave)."""
+"""k_parse latency of a lone warp per corpus class: one frame of ONE class per SM, then 32 per SM (a full wave)."""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -9,11 +9,12 @@ L = _native.lib()
 level = int(sys.argv[1]) if len(sys.argv) > 1 else 3
 ctx = ZstdBatchContext(0); ctx.setOption("timing", 1)
 dev = torch.device("cuda:0")
+sms = torch.cuda.get_device_properties(dev).multi_processor_count
 stride = (L.ZSTD_compressBound(131072) + 32 + 63) // 64 * 64
 buf = C.create_string_buffer(4096)
 stream = torch.cuda.Stream(); st = stream.cuda_stream
 for cls in range(8):
-    for n in (148, 4736):
+    for n in (sms, 32 * sms):
         data = np.stack([corpus.chunk(cls + 8 * (i % 64)) for i in range(n)])
         d_src = torch.from_numpy(data.reshape(-1)).to(dev)
         d_off = torch.arange(0, (n + 1) * 131072, 131072, dtype=torch.int64, device=dev)

@@ -1,6 +1,6 @@
-// Micro-benchmark: how many random 4-byte probes per second does the B200 memory system sustain, and how many
+// Micro-benchmark: how many random 4-byte probes per second does the H100 memory system sustain, and how many
 // DRAM bytes does each one cost, for the load flavours available in PTX and for the L2 fetch-granularity limit?
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o random_probe random_probe.cu ; run: ./random_probe [GiB]
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o random_probe random_probe.cu ; run: ./random_probe [GiB]
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

@@ -1,3 +1,4 @@
+import gzip
 import os
 import sys
 from pathlib import Path
@@ -9,7 +10,7 @@ sys.path.insert(0, str(ROOT))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: run with -m gpu)")
 
 
 @pytest.fixture(scope="session", autouse=True)
@@ -20,11 +21,19 @@ def _built():
     yield
 
 
-REFERENCE_RESOURCES = Path("/root/reference/src/test/resources")
+XML_GOLDEN = ROOT / "tests" / "golden" / "xml"
 
 
 @pytest.fixture(scope="session")
-def reference_resources():
-    if not REFERENCE_RESOURCES.exists():
-        pytest.skip("reference test resources not present on this machine")
-    return REFERENCE_RESOURCES
+def reference_resources(tmp_path_factory):
+    """The reference's test resources (zstd-jni src/test/resources) the tests decode, rebuilt from the reduced copy in
+    tests/golden/xml (tests/golden/make_golden_xml.py): the plaintext unpacked, the concatenated streams made as the
+    reference's regenerate.sh makes them."""
+    d = tmp_path_factory.mktemp("resources")
+    (d / "xml").write_bytes(gzip.decompress((XML_GOLDEN / "xml.gz").read_bytes()))
+    for f in XML_GOLDEN.iterdir():
+        if f.name != "xml.gz":
+            (d / f.name).write_bytes(f.read_bytes())
+    for name in ("xml-1", "xml-1-sized"):
+        (d / f"{name}x2.zst").write_bytes((d / f"{name}.zst").read_bytes() * 2)
+    return d

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI in include/zstdb200.h (libzstdb200.so).
 
-The library holds the sm_100a kernels; there is deliberately no fallback: if the
+The library holds the sm_90a kernels; there is deliberately no fallback: if the
 shared object is missing or no CUDA device is usable, loading / context creation
 raises, it never routes through a CPU implementation.
 """
@@ -43,7 +43,7 @@ def lib() -> C.CDLL:
     if not path.exists():
         raise NativeLibraryMissing(
             f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback.")
+            "(nvcc, sm_90a). There is no CPU fallback.")
     L = C.CDLL(str(path))
     sz, vp, i, u64 = C.c_size_t, C.c_void_p, C.c_int, C.c_uint64
 

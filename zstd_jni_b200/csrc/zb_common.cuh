@@ -1,4 +1,4 @@
-// zb_common.cuh -- shared definitions for the B200 Zstandard block codec.
+// zb_common.cuh -- shared definitions for the GPU Zstandard block codec.
 //
 // The codec is written as warp-cooperative __host__ __device__ templates over a
 // "warp context" (lane id, lane count W, sync, broadcast).  On the GPU W = 32 and

@@ -12,7 +12,7 @@ decompresses its own contiguous range of chunks.  Two shapes are supported:
     at its offset of the one contiguous stream on the root (variable-length gather) -- `gather_fixed` is the same
     for the fixed-size regenerated chunks of the decompression direction.
 
-Works on any torch.distributed backend (NCCL on the B200 box, gloo in the CPU tests).
+Works on any torch.distributed backend (NCCL between GPUs, gloo in the CPU tests).
 """
 from __future__ import annotations
 
