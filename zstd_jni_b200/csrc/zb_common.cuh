@@ -363,17 +363,21 @@ struct GroupDev {
         int const l = (int)(threadIdx.x & 31), sh = l & ~(LANES - 1);
         return GroupDev{l & (LANES - 1), (LANES >= 32) ? 0xFFFFFFFFu : (FULL << sh), sh};
     }
-    __device__ __forceinline__ void sync() const { __syncwarp(gmask); }
-    template <class T> __device__ __forceinline__ T shfl(T v, int src) const { return __shfl_sync(gmask, v, src, LANES); }
-    template <class T> __device__ __forceinline__ T bcast(T v, int src = 0) const { return __shfl_sync(gmask, v, src, LANES); }
-    __device__ __forceinline__ u32 ballot(bool p) const { return (__ballot_sync(gmask, p) >> gshift) & FULL; }
-    __device__ __forceinline__ u32 match_any(u32 v) const { return (__match_any_sync(gmask, v) >> gshift) & FULL; }
+    // A whole-warp group has a constant mask and shift.  Kernels pass the group by reference into non-inlined parsers, where
+    // the fields live on the stack and are reloaded after every global store, in front of the next collective.
+    __device__ __forceinline__ u32 mask() const { return LANES >= 32 ? 0xFFFFFFFFu : gmask; }
+    __device__ __forceinline__ int shift() const { return LANES >= 32 ? 0 : gshift; }
+    __device__ __forceinline__ void sync() const { __syncwarp(mask()); }
+    template <class T> __device__ __forceinline__ T shfl(T v, int src) const { return __shfl_sync(mask(), v, src, LANES); }
+    template <class T> __device__ __forceinline__ T bcast(T v, int src = 0) const { return __shfl_sync(mask(), v, src, LANES); }
+    __device__ __forceinline__ u32 ballot(bool p) const { return (__ballot_sync(mask(), p) >> shift()) & FULL; }
+    __device__ __forceinline__ u32 match_any(u32 v) const { return (__match_any_sync(mask(), v) >> shift()) & FULL; }
     __device__ __forceinline__ u32 sum(u32 v) const {
-        for (int o = LANES / 2; o > 0; o >>= 1) v += __shfl_xor_sync(gmask, v, o, LANES);
+        for (int o = LANES / 2; o > 0; o >>= 1) v += __shfl_xor_sync(mask(), v, o, LANES);
         return v;
     }
     __device__ __forceinline__ u32 max(u32 v) const {
-        for (int o = LANES / 2; o > 0; o >>= 1) { u32 t = __shfl_xor_sync(gmask, v, o, LANES); v = t > v ? t : v; }
+        for (int o = LANES / 2; o > 0; o >>= 1) { u32 t = __shfl_xor_sync(mask(), v, o, LANES); v = t > v ? t : v; }
         return v;
     }
     __device__ __forceinline__ void atomic_inc(u32* p) const { atomicAdd(p, 1u); }
@@ -381,7 +385,7 @@ struct GroupDev {
     // exclusive prefix sum over the group's lanes
     __device__ __forceinline__ u32 exscan(u32 v) const {
         u32 x = v;
-        for (int o = 1; o < LANES; o <<= 1) { u32 const t = __shfl_up_sync(gmask, x, o, LANES); if (lane >= o) x += t; }
+        for (int o = 1; o < LANES; o <<= 1) { u32 const t = __shfl_up_sync(mask(), x, o, LANES); if (lane >= o) x += t; }
         return x - v;
     }
     // OR one byte into memory shared with neighbouring lanes (32-bit atomic on the containing word)
@@ -392,6 +396,12 @@ struct GroupDev {
     }
 };
 typedef GroupDev<32> WarpDev;
+#endif
+// The calling lane's index in its group.  A device group derives it from the thread index instead of reading the field, which
+// lives on the stack in non-inlined parsers (and waits there behind every global store).
+template <class C> ZB_HD u32 lane_of(const C& w) { return (u32)w.lane; }
+#if defined(__CUDACC__)
+template <int LANES> __device__ __forceinline__ u32 lane_of(const GroupDev<LANES>&) { return threadIdx.x & (u32)(LANES - 1); }
 #endif
 struct WarpHost {
     int lane = 0;

@@ -303,22 +303,38 @@ ZB_HD u32 tag8(u64 d, u32 hBits) { return (u32)((d * 0xCF1BBCDCB7A56463ULL) >> (
 ZB_HD u32 tag4(u32 d) { return (d * 2246822519U) >> 18; }
 ZB_HD u32 cell(u32 idx, u32 tag) { return idx | (tag << 18); }
 
+#ifdef ZB_STATS      // host-only instrumentation (tests/hostsim builds): how much of the speculative work is useful
+// Input-stream counters (dfast): coldHeads = batches whose input loads reach a 32-byte sector beyond everything read
+// forward so far in the frame; wcReads / wcCold = wcount rounds and those reaching past that mark; near[k] = candidate and
+// repcode fetches at an offset below 1 / 2 / 4 / 6 KB / further (k = 0..4).
+struct ParseStats { unsigned long long batches, probes, useful, candL, candS, matches, bytes, frames, coldHeads, wcReads, wcCold, near[5]; };
+static ParseStats g_parseStats;
+static u32 g_statFwd;          // highest input byte + 1 read forward in the current frame
+static void stat_fwd(u32 end) { if (end > g_statFwd) g_statFwd = end; }
+static void stat_off(u32 off) { g_parseStats.near[off < 1024 ? 0 : off < 2048 ? 1 : off < 4096 ? 2 : off < 6144 ? 3 : 4]++; }
+#define ZB_STAT(x) x
+#else
+#define ZB_STAT(x)
+#endif
+
 // common prefix length of src[a..n) and src[b..) (b < a), all lanes cooperate; uniform result
 template <class C>
 ZB_HD u32 wcount(const C& w, const u8* src, u32 n, u32 a, u32 b) {
     u32 total = 0;
     u32 lanes = C::W < 8 ? C::W : 8;     // most matches are short: start with 64 bytes, then full width
+    u32 const lane = lane_of(w);
     for (;;) {
-        u32 const pa = a + total + 8u * (u32)w.lane;
-        bool const on = (u32)w.lane < lanes;
+        u32 const pa = a + total + 8u * lane;
+        bool const on = lane < lanes;
         u32 const avail = (on && pa < n) ? (n - pa < 8 ? n - pa : 8) : 0;
         u32 cnt = 0;
         if (avail) {
-            u64 const da = load64_n(src + pa, avail), db = load64_n(src + (b + total + 8u * (u32)w.lane), avail);
+            u64 const da = load64_n(src + pa, avail), db = load64_n(src + (b + total + 8u * lane), avail);
             u64 diff = da ^ db;
             if (avail < 8) diff &= (1ull << (avail * 8)) - 1;
             cnt = diff ? (ctz64(diff) >> 3) : avail;
         }
+        ZB_STAT(if (lane == 0) { u32 const e = a + total + 8 * lanes; g_parseStats.wcReads++; g_parseStats.wcCold += e > ((g_statFwd + 31) & ~31u); stat_fwd(e < n ? e : n); })
         u32 const notFull = w.ballot(!on || cnt < 8) & ((lanes >= 32) ? 0xFFFFFFFFu : ((1u << lanes) - 1));
         if (notFull) {
             u32 const f = ctz32(notFull);
@@ -332,22 +348,15 @@ ZB_HD u32 wcount(const C& w, const u8* src, u32 n, u32 a, u32 b) {
 template <class C>
 ZB_HD u32 wcatchup(const C& w, const u8* src, u32 ip, u32 m, u32 maxBack) {
     u32 total = 0;
+    u32 const lane = lane_of(w);
     for (;;) {
-        u32 const k = total + (u32)w.lane;
+        u32 const k = total + lane;
         bool const eq = (k < maxBack) && (src[ip - 1 - k] == src[m - 1 - k]);
         u32 const mask = w.ballot(eq);
         if (mask != C::FULL) return total + ctz32(~mask);
         total += C::W;
     }
 }
-
-#ifdef ZB_STATS      // host-only instrumentation (tests/hostsim builds): how much of the speculative work is useful
-struct ParseStats { unsigned long long batches, probes, useful, candL, candS, matches, bytes; };
-static ParseStats g_parseStats;
-#define ZB_STAT(x) x
-#else
-#define ZB_STAT(x)
-#endif
 
 // MLS != 0: the short table's match length is known at compile time (level 3's row has 5), so its hash is one expression, no switch
 template <class C, u32 MLS = 0>
@@ -358,12 +367,13 @@ ZB_HDN u32 parse_dfast_warp(const C& w, const EncWork& W, const u8* src, size_t 
     int ip = 1, anchor = 0;
     u32 off1 = 1, off2 = 0;             // {1,4,8} clipped by maxRep = 1 at position 1 (zstd_double_fast.c:158-164)
     u32 nbSeq = 0;
-    u32 const lane = (u32)w.lane;
+    u32 const lane = lane_of(w);
     bool rep2Pending = false;           // the "immediate repcode" test of :308-320 is due at ip (folded into the next batch)
     // Every speculative probe costs ~200 B of random HBM traffic (two table sectors read and written back, two or
     // three candidate sectors), and probes behind the first hit are wasted.  The first batch of a search phase is
     // therefore sized from a running estimate of how many positions recent phases needed; it doubles on a miss.
     u32 est4 = 4 * 3;                   // estimate x4 (fixed point)
+    ZB_STAT(if (lane == 0) { g_statFwd = 0; g_parseStats.frames++; })
     for (;;) {   // one iteration per stored match
         u32 step = 1; int nextStep = ip + 256, ip1 = ip + 1;
         if (ip1 > ilimit) {
@@ -413,13 +423,17 @@ ZB_HDN u32 parse_dfast_warp(const C& w, const EncWork& W, const u8* src, size_t 
                 bool const repOk = (off1 > 0) && (load32(src + p + 1 - (int)off1) == (u32)(d8 >> 8));
                 bool const longOk = plausL && (load64(src + (idxl - 2)) == d8);
                 bool const shortOk = plausS && (load32(src + (idxs - 2)) == (u32)d8);
-                ZB_STAT(g_parseStats.probes++; g_parseStats.candL += plausL && !lowL; g_parseStats.candS += plausS && !lowS;)
+                ZB_STAT(g_parseStats.probes++; g_parseStats.candL += plausL && !lowL; g_parseStats.candS += plausS && !lowS;
+                        if (off1 > 0) stat_off(off1); if (plausL) stat_off((u32)p + 2 - idxl); if (plausS) stat_off((u32)p + 2 - idxs);
+                        if (rep2Pending && lane == 0 && off2 > 0) stat_off(off2);)
                 kind = rep2Hit ? 4 : repOk ? 1 : longOk ? 2 : shortOk ? 3 : 0;
             }
             u32 const hm = w.ballot(kind != 0);
             nActive = popc32(w.ballot(active));
             ev = hm ? (int)ctz32(hm) : -1;
             int const last = ev >= 0 ? ev : (int)nActive - 1;
+            ZB_STAT({ u32 const e = (u32)w.shfl(p, (int)nActive - 1) + 8;
+                      if (lane == 0) { g_parseStats.coldHeads += e > ((g_statFwd + 31) & ~31u); stat_fwd(e < (u32)n ? e : (u32)n); } })
             if (active && (int)lane <= last) {
                 u32 const later = ((last >= 31) ? 0xFFFFFFFFu : ((2u << last) - 1)) & ~((2u << lane) - 1);
                 if (!(mL & later)) hashLong[hl] = cell((u32)p + 2, myTagL);
