@@ -2,8 +2,8 @@
 
 Run in the dev container (needs /root/reference to have built oracle/_ref):
     python -m tests.golden.make_golden
-The fixtures are small on purpose; inputs are regenerated from the deterministic corpus generator, only
-their SHA-256 is stored.  Nothing here runs on the GPU box except regenerate_input().
+The fixtures are small on purpose; inputs are regenerated from the deterministic corpus generator or a seeded
+generator (regenerate_input), only their SHA-256 is stored.  Nothing here runs on the GPU box except regenerate_input().
 """
 from __future__ import annotations
 
@@ -25,7 +25,125 @@ def regenerate_input(spec: dict) -> bytes:
         return dict(cases.special_cases())[spec["name"]]
     if spec["kind"] == "multi":
         return b"".join(corpus.chunk(i).tobytes() for i in spec["indices"])[: spec["size"]]
+    import numpy as np
+    if spec["kind"] == "tokens":           # random tokens of `width` bytes drawn from a vocabulary of `vocab` random tokens
+        rng = np.random.default_rng(spec["seed"])
+        voc = rng.integers(0, 256, (spec["vocab"], spec["width"]), dtype=np.uint8)
+        return voc[rng.integers(0, spec["vocab"], -(-spec["size"] // spec["width"]))].reshape(-1)[: spec["size"]].tobytes()
+    if spec["kind"] == "alphabet":         # independent bytes from the first `alpha` letters
+        rng = np.random.default_rng(spec["seed"])
+        return (rng.integers(0, spec["alpha"], spec["size"], dtype=np.uint8) + 33).tobytes()
+    if spec["kind"] == "planted":          # `copies` x (fresh bytes from an alphabet, then a copy of an earlier stretch)
+        rng = np.random.default_rng(spec["seed"])
+        out = bytearray(rng.integers(0, spec["alpha"], spec["fresh"], dtype=np.uint8).tobytes())
+        for _ in range(spec["copies"]):
+            n = int(rng.integers(8, 25)); at = int(rng.integers(0, max(1, len(out) - n)))
+            out += bytes(out[at:at + n])
+            out += rng.integers(0, spec["alpha"], int(rng.integers(1, spec["fresh"] + 1)), dtype=np.uint8).tobytes()
+        return bytes(out)
+    if spec["kind"] == "samecodes":        # `count` x (64 ... 80 fresh bytes, then 10 bytes from 61 ... 124 back): one LL / OF / ML code each
+        rng = np.random.default_rng(spec["seed"])
+        out = bytearray(rng.integers(0, 256, 40, dtype=np.uint8).tobytes())
+        for k in range(spec["count"]):
+            out += rng.integers(0, 256, int(rng.integers(64, 81)), dtype=np.uint8).tobytes()
+            d = 61 + (29 * k) % 64         # never one of the last three offsets: no repcodes
+            out += bytes(out[len(out) - d:len(out) - d + 10])
+        return bytes(out) + rng.integers(0, 256, 16, dtype=np.uint8).tobytes()      # (no match is looked for in the last bytes)
+    if spec["kind"] == "repeat":
+        return bytes([spec["byte"]]) * spec["size"]
     raise KeyError(spec["kind"])
+
+
+# ---- decode-only frames from the reference's other encoders (optimal parsers, explicit parameters), one block each
+EXPERIMENTAL_IDS = {"literalCompressionMode": 1002, "splitAfterSequences": 1010, "blockSplitterLevel": 1017}
+NO_SPLIT = {"blockSplitterLevel": 1, "splitAfterSequences": 2}      # the optimal levels split 128 KB inputs into several blocks by default
+
+
+def ref_compress_ids(data: bytes, level: int, params: dict) -> bytes:
+    """The compiled reference with explicit and experimental parameters (names of CPARAM_IDS / EXPERIMENTAL_IDS)."""
+    import ctypes as C
+    from tests.oracle_util import CPARAM_IDS, ERR_MAX, ref
+    R = ref()
+    cctx = R.ZSTD_createCCtx()
+    try:
+        R.ZSTD_CCtx_setParameter(cctx, 100, level)
+        for k, v in params.items():
+            assert R.ZSTD_CCtx_setParameter(cctx, {**CPARAM_IDS, **EXPERIMENTAL_IDS}[k], v) <= ERR_MAX, k
+        cap = len(data) + (len(data) >> 8) + 1024
+        out = C.create_string_buffer(cap)
+        n = R.ZSTD_compress2(cctx, out, cap, data, len(data))
+        assert n <= ERR_MAX
+        return out.raw[:n]
+    finally:
+        R.ZSTD_freeCCtx(cctx)
+
+
+def foreign_frames():
+    """(name, input spec, level, params, frame, note) for every foreign fixture.  Seeds are searched where a feature needs an exact
+    value; every frame is one the staged decoder takes itself (tests/golden/frame_info.py FrameInfo.staged)."""
+    from tests.golden.frame_info import EDGE_NBSEQ, parse_frame
+    out = []
+
+    def add(name, spec, level, params, frame=None, note=None):
+        data = regenerate_input(spec)
+        z = frame if frame is not None else ref_compress_ids(data, level, {**NO_SPLIT, **params})
+        assert parse_frame(z).staged, name
+        out.append((name, spec, level, params, z, note))
+        return z
+
+    def search(name, level, params, specs, want):
+        for spec in specs:
+            z = ref_compress_ids(regenerate_input(spec), level, {**NO_SPLIT, **params})
+            if want(parse_frame(z)):
+                return add(name, spec, level, params, z)
+        raise AssertionError(f"no seed reaches {name}")
+
+    # the most sequences a 128 KB block gets: random 3-byte tokens, minMatch 3 (three-byte sequence count)
+    best = None
+    for vocab in (150, 200, 256, 300):
+        spec = {"kind": "tokens", "seed": 0, "vocab": vocab, "width": 3, "size": 131070}
+        z = ref_compress_ids(regenerate_input(spec), 19, {**NO_SPLIT, "minMatch": 3})
+        if best is None or parse_frame(z).nb_seq > parse_frame(best[1]).nb_seq:
+            best = (spec, z)
+    add("L19_mm3_maxseq", best[0], 19, {"minMatch": 3}, best[1])
+    add("L22_tokens4", {"kind": "tokens", "seed": 1, "vocab": 3000, "width": 4, "size": 131072}, 22, {})
+    add("L16_tokens5", {"kind": "tokens", "seed": 2, "vocab": 2000, "width": 5, "size": 100000}, 16, {})
+    add("L13_alpha8", {"kind": "alphabet", "seed": 3, "alpha": 8, "size": 60000}, 13, {})
+    # sequence counts on the walk -> value link depth and the k_order bucket edge; raw literals (incompressible fresh bytes)
+    levels = (19, 13, 16, 22)
+    for k, n in enumerate(EDGE_NBSEQ):
+        search(f"L{levels[k % 4]}_nbseq{n}", levels[k % 4], {},
+               ({"kind": "planted", "seed": s, "alpha": 256, "fresh": 40, "copies": n} for s in range(300)), lambda i, n=n: i.nb_seq == n)
+    # Huffman literals of 8 ... 63 bytes next to 1 ... 31 sequences (btultra2 compresses literal sections from 8 bytes on)
+    for k, (n, fresh) in enumerate(((2, 8), (5, 8), (11, 6), (24, 3))):
+        search(f"L19_huf_small_{k}", 19, {},
+               ({"kind": "planted", "seed": s, "alpha": 4, "fresh": fresh, "copies": n} for s in range(300)),
+               lambda i: i.lit_mode == 2 and 8 <= i.lit_size <= 63 and 1 <= i.nb_seq <= 31)
+    # one length / offset code throughout: RLE mode in all three positions
+    search("L19_rle_tables", 19, {}, ({"kind": "samecodes", "seed": s, "count": 24} for s in range(300)),
+           lambda i: i.modes == ("rle", "rle", "rle"))
+    # literal-only compressed blocks: Huffman 255 bytes (one stream) and 256 bytes (four streams)
+    for size in (255, 256):
+        search(f"L19_huf_lit{size}", 19, {}, ({"kind": "alphabet", "seed": s, "alpha": 40, "size": size} for s in range(300)),
+               lambda i: i.lit_mode == 2 and i.nb_seq == 0)
+    search("L22_huf_lit_only", 22, {}, ({"kind": "alphabet", "seed": s, "alpha": 24, "size": 90} for s in range(300)),
+           lambda i: i.lit_mode == 2 and i.nb_seq == 0)
+    # explicit parameters: minMatch 3, a small window, literal compression disabled
+    add("L19_mm3_w12_rawlit", {"kind": "alphabet", "seed": 4, "alpha": 8, "size": 4000}, 19,
+        {"minMatch": 3, "windowLog": 12, "literalCompressionMode": 2})
+    add("L19_mm3_w10_rawlit", {"kind": "tokens", "seed": 5, "vocab": 60, "width": 3, "size": 1000}, 19,
+        {"minMatch": 3, "windowLog": 10, "literalCompressionMode": 2})
+    add("L13_mm3_rawlit_big", {"kind": "tokens", "seed": 6, "vocab": 500, "width": 3, "size": 120000}, 13,
+        {"minMatch": 3, "literalCompressionMode": 2})
+    # RLE literals next to sequences: the reference writes them only when all (>= 8) literals are one byte, which a block of one
+    # repeated byte never has (one literal, then a match); so the raw one-byte literals section of that frame is re-typed as RLE
+    spec = {"kind": "repeat", "byte": 97, "size": 1000}
+    z = bytearray(ref_compress_ids(regenerate_input(spec), 19, NO_SPLIT))
+    i = parse_frame(bytes(z)); at = i.header_size + 3
+    assert i.lit_mode == 0 and i.lit_size == 1 and z[at] == 0x08 and i.nb_seq == 1
+    z[at] = 0x09                           # literals section header: RLE, one byte
+    add("L19_rle_lit", spec, 19, {}, bytes(z), "raw literals section of the reference frame re-typed as RLE")
+    return out
 
 
 def main():
@@ -92,6 +210,19 @@ def main():
     skippable = b"\x50\x2a\x4d\x18" + (7).to_bytes(4, "little") + b"skipped"
     (HERE / "concat_skippable.zst").write_bytes(skippable + z3 + skippable + z3)
     man["decode_only"].append({"file": "concat_skippable.zst", "size": 300000, "sha256": hashlib.sha256(data[:150000] * 2).hexdigest(), "input": None})
+    from tests.golden.frame_info import REQUIRED_FEATURES, features
+    seen = set()
+    for name, spec, level, params, z, note in foreign_frames():
+        data = regenerate_input(spec)
+        fn = f"foreign_{name}.zst"
+        (HERE / fn).write_bytes(z)
+        e = {"file": fn, "size": len(data), "sha256": hashlib.sha256(data).hexdigest(), "input": spec, "level": level, "params": params,
+             "features": features(z)}
+        if note:
+            e["note"] = note
+        man["decode_only"].append(e)
+        seen |= set(e["features"])
+    assert REQUIRED_FEATURES <= seen, sorted(REQUIRED_FEATURES - seen)
     # error behaviour pinned by the reference
     base = ref_compress(regenerate_input({"kind": "corpus", "index": 1, "size": 20000}), 3)
     probes = {"err_truncated_end.zst": base[:-1], "err_truncated_mid.zst": base[: len(base) // 2], "err_bad_magic.zst": b"\x00" + base[1:],

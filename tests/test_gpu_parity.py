@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from tests import cases
+from tests.golden.frame_info import literal_payload, parse_frame
 from tests.oracle_util import oracle_compress, oracle_decompress, ref, ref_compress, ref_stream_compress
 
 pytestmark = pytest.mark.gpu
@@ -87,27 +88,188 @@ def test_decoder_matches_oracle_on_corruptions(ctx):
             if rng.random() < 0.2:
                 zz = zz[: int(rng.integers(1, len(zz)))]
             blobs.append(bytes(zz)); caps.append(len(data)); exp.append(oracle_decompress(bytes(zz), len(data)))
+    # single-block frames of the reference's optimal parsers: minMatch 3, raw literals, the most sequences the staged path sees
+    for e in _foreign_entries():
+        if e["file"] not in ("foreign_L19_mm3_maxseq.zst", "foreign_L19_mm3_w12_rawlit.zst", "foreign_L19_nbseq17.zst", "foreign_L19_huf_small_3.zst"):
+            continue
+        z = (GOLDEN / e["file"]).read_bytes()
+        for _ in range(48):
+            zz = bytearray(z)
+            k = int(rng.integers(0, len(zz))); zz[k] ^= 1 << int(rng.integers(0, 8))
+            if rng.random() < 0.2:
+                zz = zz[: int(rng.integers(1, len(zz)))]
+            blobs.append(bytes(zz)); caps.append(e["size"]); exp.append(oracle_decompress(bytes(zz), e["size"]))
     got = ctx.decompressBatch(blobs, caps, raise_on_error=False)
     for k, (e, g) in enumerate(zip(exp, got)):
         assert e == g, (k, e if isinstance(e, int) else "ok", g if isinstance(g, int) else "ok")
 
 
-def _literal_payload(z: bytes):
-    """(first, end) byte range of the compressed-literals payload (Huffman tree description + streams) of a one-block frame, or None."""
-    fhd = z[4]; single = (fhd >> 5) & 1; fcs = fhd >> 6; did = fhd & 3
-    pos = 5 + (0 if single else 1) + (4 if did == 3 else did) + ((1 << fcs) if fcs else (1 if single else 0))
-    bh = z[pos] | (z[pos + 1] << 8) | (z[pos + 2] << 16)
-    if (bh >> 1) & 3 != 2:
+def _foreign_entries():
+    """The decode-only fixtures written by the reference's optimal parsers and explicit parameters (tests/golden/make_golden.py)."""
+    man = json.loads((GOLDEN / "manifest.json").read_text())
+    return [e for e in man["decode_only"] if e["file"].startswith("foreign_")]
+
+
+def _info(z: bytes):
+    """parse_frame(z), or None where a damaged header does not parse."""
+    try:
+        return parse_frame(z)
+    except (ValueError, IndexError):
         return None
-    blk = pos + 3
-    b0 = z[blk]; typ = b0 & 3; lhl = (b0 >> 2) & 3
-    if typ < 2:
-        return None
-    lhc = int.from_bytes(z[blk:blk + 5], "little")
-    if lhl < 2: lh, csz = 3, (lhc >> 14) & 0x3FF
-    elif lhl == 2: lh, csz = 4, (lhc >> 18) & 0x3FFF
-    else: lh, csz = 5, (lhc >> 22) & 0x3FFFF
-    return blk + lh, blk + lh + csz
+
+
+def _one_block_frame(content: int, btype: int, payload: bytes) -> bytes:
+    """A single-segment frame with one last raw (btype 0) or RLE (btype 1) block, written by hand: the encoders never put an
+    RLE block first."""
+    if content < 256: fhd, fcs = 0x20, content.to_bytes(1, "little")
+    elif content < 65792: fhd, fcs = 0x60, (content - 256).to_bytes(2, "little")
+    else: fhd, fcs = 0xA0, content.to_bytes(4, "little")
+    return b"\x28\xb5\x2f\xfd" + bytes([fhd]) + fcs + (1 | (btype << 1) | (content << 3)).to_bytes(3, "little") + payload
+
+
+def _decompress_packed(ctx, blobs, caps):
+    """zstdb200_decompress_frames on the packed batch: per item the bytes or the negative error code."""
+    import ctypes as C
+    from zstd_jni_b200 import _native
+    L = _native.lib()
+    k = len(blobs)
+    stream = np.frombuffer(b"".join(blobs), dtype=np.uint8)
+    fs = (C.c_size_t * k)(*[len(b) for b in blobs])
+    ds = (C.c_size_t * k)(*caps)
+    out = np.empty(max(sum(caps), 1), dtype=np.uint8)
+    L.zstdb200_decompress_frames(ctx.handle, C.c_void_p(stream.ctypes.data), fs, k, C.c_void_p(out.ctypes.data), sum(caps), ds)
+    offs = np.concatenate([[0], np.cumsum(caps)]).astype(np.int64)
+    return [-_native.error_code(ds[i]) if _native.is_error(ds[i]) else out[offs[i]:offs[i] + ds[i]].tobytes() for i in range(k)]
+
+
+def test_staged_decoder_batches_past_the_chain_lanes():
+    """k_dec_chains runs one CTA per SM with 2 x 14 sequence walk lanes and 2 x 8 Huffman groups; every lane draws frames from a
+    longest-first list until the list holds no more work.  Here a batch of bench size or more puts twice as many items without
+    sequences as there are walk lanes (raw, RLE, empty, literal-only, checksummed, multi-block, multi-frame, no content size, damaged
+    headers) ahead of 2000 items with 1 ... 31 sequences -- some with 8 ... 63 Huffman-coded literals -- and then interleaves them 3:1.  Before every batch the same work set
+    decodes unrelated 128 KB frames, so a frame whose sequences or literals were never decoded would execute another frame's records."""
+    from collections import Counter
+    import torch
+    from zstd_jni_b200 import corpus
+    from zstd_jni_b200.zstd import ZstdBatchContext
+    from tests.golden.make_golden import regenerate_input
+    from tests.oracle_util import oracle_compress_flags
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    rng = np.random.default_rng(33)
+
+    def entry(z, data=None, cap=None):
+        cap = len(data) if cap is None else cap
+        e = oracle_decompress(z, cap)
+        if data is not None:
+            assert e == data
+        return (z, cap, e)
+
+    # items without sequences
+    zero = [entry(_one_block_frame(0, 0, b""), b""), entry(oracle_compress(b"", 3), b"")]
+    for n in (1, 17, 255, 256, 5000, 65792, 131072):
+        d = rng.integers(0, 256, n, dtype=np.uint8).tobytes()
+        zero += [entry(_one_block_frame(n, 0, d), d), entry(_one_block_frame(n, 1, d[:1]), d[:1] * n)]
+        if n <= 5000:
+            zero.append(entry(oracle_compress(d, 3), d))                                          # incompressible: a raw block
+    for e in _foreign_entries():
+        z = (GOLDEN / e["file"]).read_bytes()
+        if parse_frame(z).nb_seq == 0:
+            zero.append(entry(z, regenerate_input(e["input"])))                                       # Huffman literals only
+    for k in range(6):
+        d = corpus.chunk(k)[: 3000 + 7000 * k].tobytes()
+        zero.append(entry(oracle_compress_flags(d, 3, checksum=True), d))
+        zero.append(entry(oracle_compress_flags(d, 1, content_size=False), d))
+        zero.append(entry(oracle_compress(d, 3) + oracle_compress(d[:999], 1), d + d[:999]))      # two frames in one item
+    man = json.loads((GOLDEN / "manifest.json").read_text())
+    e = next(e for e in man["decode_only"] if e["file"] == "stream_L1.zst")
+    zero.append(entry((GOLDEN / e["file"]).read_bytes(), regenerate_input(e["input"])))             # several blocks
+    for k in range(24):
+        z = bytearray(oracle_compress(corpus.chunk(k)[:20000].tobytes(), 1 + 2 * (k % 2)))
+        at = parse_frame(bytes(z)).header_size + 3 + int(rng.integers(0, 4))                        # literals / sequences header damaged
+        z[at] ^= 1 << int(rng.integers(0, 8))
+        zero.append(entry(bytes(z), cap=20000))
+    zero = [t for t in zero if _info(t[0]) is None or _info(t[0]).nb_seq == 0 or not _info(t[0]).staged]
+    # items with 1 ... 31 sequences
+    small = []
+    for e in _foreign_entries():
+        z = (GOLDEN / e["file"]).read_bytes()
+        if 1 <= parse_frame(z).nb_seq <= 31:
+            small.append(entry(z, regenerate_input(e["input"])))
+    for s in range(60):
+        d = regenerate_input({"kind": "planted", "seed": 100 + s, "alpha": 256 if s % 2 else 16, "fresh": 30, "copies": 1 + s % 30})
+        z = oracle_compress(d, 1 + 2 * (s % 2))
+        if 1 <= parse_frame(z).nb_seq <= 31:
+            small.append(entry(z, d))
+    huf_small = [t for t in small if parse_frame(t[0]).lit_mode == 2 and parse_frame(t[0]).lit_size < 64]
+    assert len(small) >= 40 and len(huf_small) >= 4
+
+    n_zero, n_small = 2 * 28 * sms, 2000
+    n = max(8192, n_zero + n_small)
+    n_zero = n - n_small
+    zeros = [zero[k % len(zero)] for k in range(n_zero)]
+    smalls = [small[k % len(small)] for k in range(n_small)]
+    no_huf = sum(1 for t in zeros if _info(t[0]) is None or _info(t[0]).lit_mode != 2 or not _info(t[0]).staged)
+    assert no_huf >= 2 * 16 * sms
+    first = zeros + smalls
+    inter, zi, si = [], iter(zeros), iter(smalls)
+    for k in range(n):
+        inter.append(next(si, None) if k % 4 == 3 else next(zi, None))
+    inter = [t for t in inter if t is not None] + list(zi) + list(si)
+
+    stale_data = [corpus.chunk(300 + k).tobytes() for k in range(64)]
+    stale = [oracle_compress(stale_data[k], 3) for k in range(64)] * (n // 64 + 1)
+    stale = stale[:n]
+    failures = []
+    c = ZstdBatchContext(0)
+    try:
+        c.setOption("host_slices_dec", 1)            # the packed call decodes the whole batch at once, on the same work set
+        for name, batch in (("sequence-free first", first), ("interleaved 3:1", inter)):
+            blobs, caps, exp = [t[0] for t in batch], [t[1] for t in batch], [t[2] for t in batch]
+            got = {}
+            for pipeline in (1, 0):
+                c.setOption("dec_pipeline", pipeline)
+                assert all(o == stale_data[k % 64] for k, o in enumerate(c.decompressBatch(stale, [131072] * n)))
+                got[pipeline] = c.decompressBatch(blobs, caps, raise_on_error=False)
+            c.setOption("dec_pipeline", 1)
+            assert all(o == stale_data[k % 64] for k, o in enumerate(c.decompressBatch(stale, [131072] * n)))
+            got["packed"] = _decompress_packed(c, blobs, caps)
+            for how, g in got.items():
+                wrong = [g[k] for k in range(n) if g[k] != exp[k]]
+                if wrong:
+                    codes = Counter(w if isinstance(w, int) else "bytes" for w in wrong)
+                    failures.append(f"{name}, {'packed' if how == 'packed' else f'dec_pipeline {how}'}: {len(wrong)} of {n} items differ from the "
+                                    f"oracle, results {dict(codes)}")
+    finally:
+        c.close()
+    assert not failures, failures
+
+
+def test_staged_decoder_at_every_stream_alignment():
+    """The staged decoder counts a stream's words from the 16-byte boundary at or below its first byte and masks the first word.  A
+    hand-written raw-block frame of chosen size in front of every foreign fixture puts it at all 16 source offsets (and moves its
+    destination with it)."""
+    from tests.golden.make_golden import regenerate_input
+    rng = np.random.default_rng(44)
+    blobs, caps, want = [], [], []
+    pos = 0
+    for e in _foreign_entries():
+        z = (GOLDEN / e["file"]).read_bytes()
+        data = regenerate_input(e["input"])
+        for s in range(16):
+            p = (s - pos - 9) % 16                   # a 9-byte header, then p bytes: the fixture starts at pos + 9 + p = s (mod 16)
+            filler = rng.integers(0, 256, p, dtype=np.uint8).tobytes()
+            f = _one_block_frame(p, 0, filler)
+            assert len(f) == 9 + p
+            blobs += [f, z]; caps += [p, len(data)]; want += [filler, data]
+            pos += len(f) + len(z)
+            assert (pos - len(z)) % 16 == s
+    from zstd_jni_b200.zstd import ZstdBatchContext
+    with ZstdBatchContext(0) as c:
+        for pipeline in (1, 0):
+            c.setOption("dec_pipeline", pipeline)
+            got = c.decompressBatch(blobs, caps, raise_on_error=False)
+            bad = [(k // 32, k % 32 // 2) for k in range(len(got)) if got[k] != want[k]]
+            assert not bad, (pipeline, len(bad), bad[:8])
 
 
 @pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
@@ -124,7 +286,7 @@ def test_decoder_matches_the_compiled_reference_on_corruptions(ctx):
         data = corpus.chunk(idx)[:60000].tobytes()
         for level in (3, 1):
             z = ref_compress(data, level)
-            lit = _literal_payload(z)
+            lit = literal_payload(z)
             for _ in range(40):
                 zz = bytearray(z)
                 k = int(rng.integers(0, len(zz))); zz[k] ^= 1 << int(rng.integers(0, 8))

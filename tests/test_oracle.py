@@ -43,6 +43,31 @@ def test_committed_golden_vectors():
         assert oracle_decompress(frame, e["cap"]) == -e["code"], e["file"]
 
 
+def test_foreign_fixtures_cover_the_staged_decoder_features():
+    """The decode-only frames of the reference's optimal parsers and explicit parameters: every one is a frame the staged decoder takes
+    itself, its tags in the manifest are what its bytes say (tests/golden/frame_info.py), and together they reach every listed feature."""
+    from tests.golden.frame_info import REQUIRED_FEATURES, decode_sequences, features, parse_frame
+    man = json.loads((GOLDEN / "manifest.json").read_text())
+    seen = set()
+    for e in man["decode_only"]:
+        if "features" not in e:
+            continue
+        z = (GOLDEN / e["file"]).read_bytes()
+        assert parse_frame(z).staged, e["file"]
+        assert features(z) == e["features"], e["file"]
+        seen |= set(e["features"])
+    assert REQUIRED_FEATURES <= seen, sorted(REQUIRED_FEATURES - seen)
+    # the parser itself, on frames of known content: the sequences add up (decode_sequences checks it) and the literal sizes agree
+    from tests.golden.make_golden import regenerate_input
+    for e in man["oneshot"][::7]:
+        z = (GOLDEN / e["file"]).read_bytes()
+        info = parse_frame(z)
+        assert info.content_size == len(regenerate_input(e["input"])), e["file"]
+        if info.one_block and info.block_type == 2:
+            seqs = decode_sequences(z)
+            assert len(seqs) == info.nb_seq and sum(s[0] for s in seqs) <= info.lit_size, e["file"]
+
+
 @pytest.mark.skipif(ref() is None, reason="oracle/_ref not built (no reference sources here)")
 @pytest.mark.parametrize("level", [1, 2, 3, 4, -1, -5, 5, 6, 7, 9, 10, 12])
 def test_oracle_matches_compiled_reference(level):

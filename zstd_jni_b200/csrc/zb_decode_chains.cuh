@@ -174,7 +174,7 @@ __device__ __forceinline__ void chains_walk_warp(const ChainsArgs& a, unsigned c
                 item = a.orderSeq[item];
                 d = a.descs + item;
                 u32 const nbSeq = d->nbSeq;
-                if (nbSeq == 0) exhausted = true;            // longest first: only frames without sequences from here on
+                if (nbSeq == 0) exhausted = true;            // k_order puts every frame without sequences after all others: none left
                 else if (d->mode == 1 && !d->stA1 && !d->stA2 && !d->seqUnusable) {
                     u32 const logLL = d->logLL, logOF = d->logOF, logML = d->logML;
                     u32 const bLL = umax(16u, 4u << logLL), bOF = umax(16u, 4u << logOF), bML = umax(16u, 4u << logML);
@@ -301,7 +301,7 @@ __device__ __forceinline__ void chains_huf_warp(const ChainsArgs& a, unsigned ch
             if (item == 0xFFFFFFFFu) exhausted = true;
             else {
                 d = a.descs + item;
-                if (d->hufLitSize == 0) exhausted = true;    // longest first: no Huffman-coded literals from here on
+                if (d->hufLitSize == 0) exhausted = true;    // k_order puts every frame without Huffman literals last: none left
                 else if (d->mode == 1 && !d->stA1 && d->litMode == 2) {
                     u32 const log = d->hufLog;
                     __syncwarp(gmask);                         // the siblings' last reads of the slot's old table come first
