@@ -11,7 +11,8 @@ import pytest
 
 from tests import cases
 from tests.golden.frame_info import literal_payload, parse_frame
-from tests.oracle_util import oracle_compress, oracle_decompress, ref, ref_compress, ref_stream_compress
+from tests.oracle_util import (oracle_compress, oracle_compress_flags, oracle_decompress, ref, ref_compress, ref_compress_flags,
+                               ref_stream_compress)
 
 pytestmark = pytest.mark.gpu
 GOLDEN = Path(__file__).parent / "golden"
@@ -26,21 +27,27 @@ def ctx():
 
 
 def _expected(data, level):
+    """The oracle's frame, or its negative error code where it refuses (parameter_unsupported for inputs of 16 KB or less at levels
+    11 and 12, which select the optimal parser there); a frame must equal the compiled reference's when oracle/_ref is built."""
     r = oracle_compress(data, level)
-    if ref() is not None:
+    if ref() is not None and not isinstance(r, int):
         assert ref_compress(data, level) == r
     return r
 
 
-@pytest.mark.parametrize("level", [3, 1, 4, 2, -1, 5, 7, 9, 12])
+@pytest.mark.parametrize("level", [3, 1, 4, 2, -1, 5, 7, 9, 12, 6, 8, 10, 11, -2, -5, -50, -131072])
 def test_compress_bit_exact_vs_oracle(ctx, level):
+    """Every level the README calls bit-exact, -131072 included (the fast parser with a step wider than a block).  At levels 11 and 12
+    the same batch holds inputs of 16 KB or less, which must fail alone with parameter_unsupported while the others are written."""
     todo = cases.special_cases() + cases.corpus_cases(32) + cases.edge_cases()
-    if level >= 11:
-        todo = [t for t in todo if len(t[1]) > 16384]
-    frames = ctx.compressBatch([d for _, d in todo], level)
+    frames = ctx.compressBatch([d for _, d in todo], level, raise_on_error=False)
     assert ctx.kernelLaunches() > 0
+    refused = 0
     for (name, data), got in zip(todo, frames):
-        assert got == _expected(data, level), (name, level)
+        exp = _expected(data, level)
+        assert got == exp, (name, level, got if isinstance(got, int) else len(got), exp if isinstance(exp, int) else len(exp))
+        refused += exp == -40
+    assert refused == (sum(len(d) <= 16384 for _, d in todo) if level >= 11 else 0)
 
 
 def test_unsupported_levels_fail_loudly(ctx):
@@ -142,19 +149,13 @@ def _decompress_packed(ctx, blobs, caps):
     return [-_native.error_code(ds[i]) if _native.is_error(ds[i]) else out[offs[i]:offs[i] + ds[i]].tobytes() for i in range(k)]
 
 
-def test_staged_decoder_batches_past_the_chain_lanes():
-    """k_dec_chains runs one CTA per SM with 2 x 14 sequence walk lanes and 2 x 8 Huffman groups; every lane draws frames from a
-    longest-first list until the list holds no more work.  Here a batch of bench size or more puts twice as many items without
-    sequences as there are walk lanes (raw, RLE, empty, literal-only, checksummed, multi-block, multi-frame, no content size, damaged
-    headers) ahead of 2000 items with 1 ... 31 sequences -- some with 8 ... 63 Huffman-coded literals -- and then interleaves them 3:1.  Before every batch the same work set
-    decodes unrelated 128 KB frames, so a frame whose sequences or literals were never decoded would execute another frame's records."""
-    from collections import Counter
-    import torch
+def _staged_decoder_items():
+    """Decode items as (frame, capacity, oracle result): those without sequences (raw, RLE, empty, literal-only, checksummed,
+    multi-block, multi-frame, no content size, damaged headers) and those with 1 ... 31 sequences, some with 8 ... 63 Huffman-coded
+    literals."""
     from zstd_jni_b200 import corpus
-    from zstd_jni_b200.zstd import ZstdBatchContext
     from tests.golden.make_golden import regenerate_input
     from tests.oracle_util import oracle_compress_flags
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
     rng = np.random.default_rng(33)
 
     def entry(z, data=None, cap=None):
@@ -202,6 +203,29 @@ def test_staged_decoder_batches_past_the_chain_lanes():
             small.append(entry(z, d))
     huf_small = [t for t in small if parse_frame(t[0]).lit_mode == 2 and parse_frame(t[0]).lit_size < 64]
     assert len(small) >= 40 and len(huf_small) >= 4
+    return zero, small
+
+
+def _interleave_3_1(zeros, smalls):
+    """Three items of `zeros`, then one of `smalls`, ...; whichever list is longer ends the batch."""
+    inter, zi, si = [], iter(zeros), iter(smalls)
+    for k in range(len(zeros) + len(smalls)):
+        inter.append(next(si, None) if k % 4 == 3 else next(zi, None))
+    return [t for t in inter if t is not None] + list(zi) + list(si)
+
+
+def test_staged_decoder_batches_past_the_chain_lanes():
+    """k_dec_chains runs one CTA per SM with 2 x 14 sequence walk lanes and 2 x 8 Huffman groups; every lane draws frames from a
+    longest-first list until the list holds no more work.  Here a batch of bench size or more puts twice as many items without
+    sequences as there are walk lanes ahead of 2000 items with 1 ... 31 sequences (_staged_decoder_items) and then interleaves them
+    3:1.  Before every batch the same work set decodes unrelated 128 KB frames, so a frame whose sequences or literals were never
+    decoded would execute another frame's records."""
+    from collections import Counter
+    import torch
+    from zstd_jni_b200 import corpus
+    from zstd_jni_b200.zstd import ZstdBatchContext
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    zero, small = _staged_decoder_items()
 
     n_zero, n_small = 2 * 28 * sms, 2000
     n = max(8192, n_zero + n_small)
@@ -211,10 +235,7 @@ def test_staged_decoder_batches_past_the_chain_lanes():
     no_huf = sum(1 for t in zeros if _info(t[0]) is None or _info(t[0]).lit_mode != 2 or not _info(t[0]).staged)
     assert no_huf >= 2 * 16 * sms
     first = zeros + smalls
-    inter, zi, si = [], iter(zeros), iter(smalls)
-    for k in range(n):
-        inter.append(next(si, None) if k % 4 == 3 else next(zi, None))
-    inter = [t for t in inter if t is not None] + list(zi) + list(si)
+    inter = _interleave_3_1(zeros, smalls)
 
     stale_data = [corpus.chunk(300 + k).tobytes() for k in range(64)]
     stale = [oracle_compress(stale_data[k], 3) for k in range(64)] * (n // 64 + 1)
@@ -415,3 +436,171 @@ def test_device_resident_api(ctx):
     assert (np.diff(ooff) == sizes).all()
     for i in (0, 1, 7, 150, 299):
         assert packed[ooff[i]:ooff[i + 1]].tobytes() == oracle_compress(data[i].tobytes(), 3)
+
+
+def _resident_parse_groups(level):
+    """Frames k_parse starts at once (32 lanes per frame, 4 frames per CTA): 8 CTAs per SM, or 6 for the lazy parser that levels 5 and up
+    run.  A larger batch is parsed in the order of a cost estimate, and its entropy stage takes frames as their parse finishes."""
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    return (24 if level >= 5 else 32) * sms
+
+
+# boundaries of the parse: empty and 1 ... 6 bytes, under 64 bytes (cost 0, the last k_order bucket), the 4 KB cut-off of the cost
+# estimate (srcSize >> 6 at or below it, a prefix parse above), the 16 KB row of the parameter table, 128 KB
+_GRID_SIZES = [0, 1, 2, 3, 4, 5, 6, 7, 31, 63, 64, 65, 200, 1000, 4095, 4096, 4097, 6000, 12000, 16383, 16384, 16385, 40000, 131071, 131072]
+
+
+def _distinct_inputs(n, sizes, seed, small=None):
+    """n inputs, no two alike where their size allows: corpus chunks cut at a varying offset with the input's index written into four of
+    their bytes, so a frame that picked up another frame's records would come out different.  Sweeps over `sizes` alternate with sweeps
+    of random sizes in `small` (a range, or None for the same list).  One sweep in ten is all one byte (RLE blocks) and another one
+    uniform random bytes (raw blocks)."""
+    from zstd_jni_b200 import corpus
+    rng = np.random.default_rng(seed)
+    base = [corpus.chunk(1000 * seed + j).tobytes() for j in range(64)]
+    out = []
+    for k in range(n):
+        sweep = k // len(sizes)
+        size = sizes[k % len(sizes)] if small is None or sweep % 2 == 0 else int(rng.integers(*small))
+        kind = sweep % 10
+        if kind == 4:
+            out.append(bytes([sweep // 10 % 255 + 1]) * size)
+            continue
+        if kind == 8:
+            out.append(rng.integers(0, 256, size, dtype=np.uint8).tobytes())
+            continue
+        src = base[k % 64]
+        at = (k * 7919) % (len(src) - size + 1)
+        d = bytearray(src[at:at + size])
+        stamp = k.to_bytes(4, "little")[:size]
+        p = (k * 31) % (size - len(stamp) + 1)
+        d[p:p + len(stamp)] = stamp
+        out.append(bytes(d))
+    return out
+
+
+def _expected_flags(data, level, checksum, content_size):
+    r = oracle_compress_flags(data, level, checksum=checksum, content_size=content_size)
+    if ref() is not None and not isinstance(r, int):
+        assert ref_compress_flags(data, level, checksum=checksum, content_size=content_size) == r
+    return r
+
+
+def _differences(got, exp):
+    bad = [k for k in range(len(exp)) if got[k] != exp[k]]
+    return len(bad), bad[:8]
+
+
+@pytest.mark.parametrize("level", [1, 3, 4, 9])
+def test_compress_past_the_resident_parse_grid(level):
+    """A batch larger than the frames k_parse holds at once takes the ordered path: the estimate pass of k_parse over a 2 KB prefix
+    (into the same table and sequence workspaces), k_order on its costs and the entropy stage fed from the completion queue.  Level 1
+    runs the fast-parser kernel, 3 the double-fast one, 4 the generic one (its 16 KB row is greedy) and 9 the lazy one.  Before every
+    checked batch the context compresses unrelated inputs at the same level, so stale sequence, meta and slot workspaces cannot pass
+    for right ones.  Every frame is compared with the oracle under the default settings, without the order, without the overlapped
+    entropy stage, with a checksum and no content size, and magicless; the launch count proves which path ran."""
+    from zstd_jni_b200 import corpus
+    from zstd_jni_b200.zstd import ZstdBatchContext
+    resident = _resident_parse_groups(level)
+    n = resident + max(1000, resident // 4)
+    datas = _distinct_inputs(n, _GRID_SIZES, 7 + level, small=(8, 20000))
+    plain = [_expected(d, level) for d in datas]
+    flagged = [_expected_flags(d, level, True, False) for d in datas]
+    magicless = [z[4:] for z in plain]                    # a magicless frame is the frame minus its magic number
+    stale_pool = [corpus.chunk(500 + j)[: (131072, 40000, 7000, 300)[j % 4]].tobytes() for j in range(16)]
+    stale = [stale_pool[k % 16] for k in range(n)]
+    runs = [("default", {}, plain, 4), ("parse_order 0", {"parse_order": 0}, plain, 2),
+            ("entropy_overlap 0", {"entropy_overlap": 0}, plain, 5),          # estimate, order, parse, order, entropy
+            ("checksum, no content size", {"checksum": 1, "content_size": 0}, flagged, 4),
+            ("magicless", {"magicless": 1}, magicless, 4)]
+    failures = []
+    with ZstdBatchContext(0) as c:
+        for name, opts, exp, launches in runs:
+            c.compressBatch(stale, level)
+            for k, v in opts.items():
+                c.setOption(k, v)
+            before = c.kernelLaunches()
+            got = c.compressBatch(datas, level)
+            assert c.kernelLaunches() - before == launches, (name, level, c.kernelLaunches() - before)
+            for k, v in opts.items():
+                c.setOption(k, {"parse_order": 1, "entropy_overlap": 1, "checksum": 0, "content_size": 1, "magicless": 0}[k])
+            wrong, first = _differences(got, exp)
+            if wrong:
+                failures.append(f"{name}: {wrong} of {n} frames differ from the oracle, first at {first}")
+    assert not failures, (level, failures)
+
+
+def _split_inputs(level):
+    """Small distinct inputs (64 B ... 6 KB), enough for a second launch part that is also ordered."""
+    n = 16384 + _resident_parse_groups(level) + 500
+    return _distinct_inputs(n, [64, 65, 100, 1000, 2047, 2048, 2049, 4095, 4096, 4097, 6000, 6144], 20 + level, small=(64, 6145))
+
+
+@pytest.mark.parametrize("level", [1, 3])
+def test_compress_past_the_launch_split(level):
+    """Batches of more than 16384 frames run as consecutive launch parts with shifted offset and size views, their own counters and
+    queues, and reused workspaces; here both parts take the ordered path.  Through the batch call every frame must equal the oracle's;
+    through the chunked call (2048-byte chunks; one slice cut into two parts, and three slices) every size, the packed stream and its
+    decoding by the oracle must be right."""
+    from zstd_jni_b200.zstd import ZstdBatchContext
+    datas = _split_inputs(level)
+    n = len(datas)
+    exp = [_expected(d, level) for d in datas]
+    with ZstdBatchContext(0) as c:
+        before = c.kernelLaunches()
+        got = c.compressBatch(datas, level)
+        assert c.kernelLaunches() - before == 8          # two ordered parts: estimate, order, parse, entropy each
+        assert _differences(got, exp) == (0, []), level
+
+    chunk = 2048
+    flat = bytearray(b"".join(d[:chunk].ljust(chunk, b"\x00") for d in datas))
+    for k in range(n):                                   # the chunks of the flat input must differ too
+        flat[k * chunk + 1000:k * chunk + 1004] = k.to_bytes(4, "little")
+    flat = bytes(flat[: n * chunk - 777])                # a short last chunk
+    pieces = [flat[k:k + chunk] for k in range(0, len(flat), chunk)]
+    assert len(pieces) == n
+    exp = [_expected(p, level) for p in pieces]
+    for slices in (1, 3):
+        with ZstdBatchContext(0) as c:
+            c.setOption("host_slices", slices)
+            stream, sizes = c.compressChunks(np.frombuffer(flat, dtype=np.uint8), chunk, level)
+        assert [int(s) for s in sizes] == [len(z) for z in exp], slices
+        assert stream.tobytes() == b"".join(exp), slices
+        assert oracle_decompress(stream.tobytes(), len(flat)) == flat, slices
+
+
+def test_decompress_past_the_launch_split():
+    """More than 16384 items in one call run as consecutive launch parts of the staged and the fused decoder: the oracle's frames of
+    the split inputs at levels 1 and 3, with the 3:1 mix of items without and with few sequences at both ends.  Every item's bytes or
+    error code must equal the oracle's, through the batch call with and without the staged decoder and through the packed call in one
+    slice (two parts) and in two."""
+    from collections import Counter
+    from zstd_jni_b200.zstd import ZstdBatchContext
+    items = []
+    for level in (1, 3):
+        for d in _split_inputs(level)[level // 2::2]:
+            items.append((oracle_compress(d, level), len(d), d))
+    zero, small = _staged_decoder_items()
+    mix = _interleave_3_1([zero[k % len(zero)] for k in range(3000)], [small[k % len(small)] for k in range(1000)])
+    batch = mix[:2000] + items + mix[2000:]
+    assert len(batch) > 16384 + 2000
+    blobs, caps, exp = [t[0] for t in batch], [t[1] for t in batch], [t[2] for t in batch]
+    for k in range(2000, 2000 + len(items)):
+        assert oracle_decompress(blobs[k], caps[k]) == exp[k]
+    got = {}
+    with ZstdBatchContext(0) as c:
+        for pipeline in (1, 0):
+            c.setOption("dec_pipeline", pipeline)
+            got[f"dec_pipeline {pipeline}"] = c.decompressBatch(blobs, caps, raise_on_error=False)
+        c.setOption("dec_pipeline", 1)
+        for slices in (1, 2):
+            c.setOption("host_slices_dec", slices)
+            got[f"packed, host_slices_dec {slices}"] = _decompress_packed(c, blobs, caps)
+    failures = []
+    for how, g in got.items():
+        wrong = [k for k in range(len(batch)) if g[k] != exp[k]]
+        if wrong:
+            codes = Counter(g[k] if isinstance(g[k], int) else "bytes" for k in wrong)
+            failures.append(f"{how}: {len(wrong)} of {len(batch)} items differ from the oracle, first at {wrong[:8]}, results {dict(codes)}")
+    assert not failures, failures

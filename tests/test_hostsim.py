@@ -14,7 +14,7 @@ from tests.oracle_util import (emu_compress, emu_decompress, hostsim_compress, h
 GOLDEN = Path(__file__).parent / "golden"
 
 
-@pytest.mark.parametrize("level", [3, 1, 4, 2, -1, -7, 5, 6, 9, 12])
+@pytest.mark.parametrize("level", [3, 1, 4, 2, -1, -7, -131072, 5, 6, 9, 12])
 def test_hostsim_encoder_matches_oracle(level):
     todo = cases.special_cases() + cases.corpus_cases(16) + cases.edge_cases(classes=(0, 2, 4, 5, 7))
     if level >= 5:       # lazy levels (row match finder): keep the CPU suite short, the big inputs are what they are for
@@ -152,7 +152,7 @@ def test_randomised_levels_and_sizes():
             parts.append(make(int(rng.integers(0, 3)), ln)); left -= ln
         return b"".join(parts)
 
-    levels = [-7, -1, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12]
+    levels = [-131072, -7, -1, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12]
     for it in range(48):
         n = int(rng.choice([rng.integers(0, 300), rng.integers(300, 16385), rng.integers(16385, 131073), 131072]))
         data = make(int(rng.integers(0, 4)), n)

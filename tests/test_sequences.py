@@ -198,3 +198,37 @@ def test_gpu_sequence_producer_inside_reference_libzstd():
         assert f(None, out.ctypes.data, 64, small, 6, None, 0, 3, 1 << 17) == (1 << 64) - 1
     finally:
         prod.freeState(state)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("level", [1, 3])
+def test_gpu_generate_sequences_past_the_launch_split(level):
+    """More than 16384 blocks in one call: the parse and the export run one launch part at a time, each part's records copied out
+    before the next part parses into the same workspaces.  Every block's records must equal the compiled reference's (or, without
+    it, the host instantiation's) and replay the block."""
+    from zstd_jni_b200 import corpus
+    from zstd_jni_b200.zstd import ZstdBatchContext
+    rng = np.random.default_rng(60 + level)
+    base = [corpus.chunk(j).tobytes() for j in range(64)]
+    blocks = []
+    for k in range(16384 + 300):
+        size = int(rng.integers(7, 1500))
+        src = base[k % 64]
+        at = int(rng.integers(0, len(src) - size + 1))
+        b = bytearray(src[at:at + size])
+        b[size // 2:size // 2 + 4] = k.to_bytes(4, "little")[: size - size // 2]       # no two blocks alike
+        blocks.append(bytes(b))
+    with ZstdBatchContext(0) as ctx:
+        before = ctx.kernelLaunches()
+        got = ctx.generateSequences(blocks, level)
+        # first part: estimate, order, parse, export; the 300-block second part is unordered: parse, export
+        assert ctx.kernelLaunches() - before == 6
+    expect = ref_generate_sequences if ref() is not None else hostsim_generate_sequences
+    bad = []
+    for k, (data, g) in enumerate(zip(blocks, got)):
+        e = expect(data, level)
+        if g.shape != e.shape or not (g == e).all():
+            bad.append(k)
+            continue
+        _check_valid_parse(g, data)
+    assert not bad, (level, len(bad), bad[:8])
