@@ -200,7 +200,11 @@ ZSTDB200_API size_t zstdb200_decompress_frames(zstdb200_ctx* ctx, const void* sr
  * costs max(kernels, copies) per batch instead of their sum.  This is what a JNI stream loop over direct buffers
  * (N/jni_outputstream_zstd.c:59-123, N/jni_directbuffercompress_zstd.c) or bench.py's end-to-end leg drives.  Buffers must stay
  * valid and untouched between begin and end; page-locked memory (cudaHostAlloc, or zstdb200_host_register on a direct
- * buffer) makes the copies truly asynchronous.  One operation per slot at a time; a context is still single-threaded. */
+ * buffer) makes the copies truly asynchronous.  One operation per slot at a time; a context is still single-threaded.
+ * The synchronous calls run on the same work sets: compress_chunks and decompress_frames on set 0, and on set 1 too when they cut
+ * the batch into slices ("host_slices" / "host_slices_dec", batches of at least 512 frames); compress_batch, decompress_batch and
+ * generate_sequences on set 0.  While a `_begin` is pending on a set such a call needs, the call returns ZSTD_error_stage_wrong
+ * and changes nothing. */
 #define ZSTDB200_SLOTS 4
 ZSTDB200_API size_t zstdb200_compress_chunks_begin(zstdb200_ctx* ctx, int slot, int level, const void* src, size_t srcSize, size_t chunkSize);
 ZSTDB200_API size_t zstdb200_compress_chunks_end(zstdb200_ctx* ctx, int slot, void* dst, size_t dstCapacity, size_t* frameSizes, size_t* dstSize);

@@ -290,6 +290,57 @@ def test_overlapped_stages_and_kernel_fifo_keep_the_bytes():
         assert o0[:t0].tobytes() == want.tobytes() == o1[:t1].tobytes()
 
 
+def test_synchronous_calls_refuse_a_busy_work_set():
+    """The synchronous and scattered-buffer calls use work set 0 (and 1 when sliced).  While a _begin is pending there they are
+    refused with stage_wrong instead of overwriting its metadata and workspaces, and the pending operation still delivers its bytes."""
+    import ctypes as C
+    import numpy as np
+    from zstd_jni_b200 import corpus
+    from zstd_jni_b200.zstd import ZstdBatchContext, ZstdException
+    n = 40
+    data = corpus.corpus(n).reshape(-1)
+    small = np.ascontiguousarray(data[: 600 * 1024])      # 600 chunks of 1 KB: two slices with host_slices 2
+    with ZstdBatchContext(0) as ctx:
+        want, fw = ctx.compressChunks(data, 131072, 3)
+        ctx.compressChunksBegin(0, data, 131072, 3)
+        for call in (lambda: ctx.compressChunks(data, 131072, 3), lambda: ctx.decompressFrames(want, fw, [131072] * n),
+                     lambda: ctx.compressBatch([data[:131072].tobytes()], 3)):
+            with pytest.raises(ZstdException) as ei:
+                call()
+            assert ei.value.getErrorCode() == 60              # stage_wrong
+        out = np.empty(data.size + 65536, dtype=np.uint8); sizes = (C.c_size_t * n)()
+        total = ctx.compressChunksEnd(0, out, sizes)
+        assert out[:total].tobytes() == want.tobytes() and list(sizes) == [int(x) for x in fw]
+        again, fa = ctx.compressChunks(data, 131072, 3)
+        assert again.tobytes() == want.tobytes()
+        back, _ = ctx.decompressFrames(again, fa, [131072] * n)
+        assert (back == data).all()
+        # a sliced call also needs work set 1; a call in one slice does not
+        ctx.setOption("host_slices", 2)
+        s1, _ = ctx.compressChunks(small, 1024, 1)
+        ctx.compressChunksBegin(1, data, 131072, 3)
+        with pytest.raises(ZstdException) as ei:
+            ctx.compressChunks(small, 1024, 1)
+        assert ei.value.getErrorCode() == 60
+        ctx.setOption("host_slices", 1)
+        assert ctx.compressChunks(small, 1024, 1)[0].tobytes() == s1.tobytes()
+        total = ctx.compressChunksEnd(1, out)
+        assert out[:total].tobytes() == want.tobytes()
+
+
+def test_decompress_frames_refuses_wrapping_sizes():
+    """Frame sizes whose sum wraps around 2^64 are refused with srcSize_wrong before a copy or a kernel: the offsets they give would
+    point outside the input."""
+    import numpy as np
+    from zstd_jni_b200.zstd import ZstdBatchContext, ZstdException
+    with ZstdBatchContext(0) as ctx:
+        before = ctx.kernelLaunches()
+        with pytest.raises(ZstdException) as ei:
+            ctx.decompressFrames(np.zeros(64, dtype=np.uint8), [1 << 63, 1 << 63], [1, 1])
+        assert ei.value.getErrorCode() == 72                  # srcSize_wrong
+        assert ctx.kernelLaunches() == before
+
+
 def test_input_stream_reads_reference_golden(reference_resources):   # Zstd.scala:426-446
     from zstd_jni_b200.zstd import ZstdInputStream
     xml = (reference_resources / "xml").read_bytes()
