@@ -221,7 +221,7 @@ ZSTDB200_API size_t zstdb200_compress_batch(zstdb200_ctx* ctx, int level, size_t
 ZSTDB200_API size_t zstdb200_decompress_batch(zstdb200_ctx* ctx, size_t n, const void* const* src, const size_t* srcSize,
                                               void* const* dst, const size_t* dstCapacity, size_t* dstSize);
 
-/* ---- entry points of features that are not built, kept here because they take THIS library's contexts (see zb_capi.cu): dictionaries
+/* ---- entry points of features that are not built, kept here because they take THIS library's contexts (see zb_libzstd.cpp): dictionaries
  * (N/jni_zstd.c:271-346, N/jni_fast_zstd.c:133-250,325-362,673-710) and foreign sequence producers (N/jni_zstd.c:337-346).  A non-empty
  * dictionary / non-NULL CDict or DDict is refused with ZSTD_error_parameter_unsupported, clearing calls succeed; after
  * ZSTD_registerSequenceProducer(cctx, state, fn != NULL) compressions of that context report parameter_unsupported until it is cleared. */

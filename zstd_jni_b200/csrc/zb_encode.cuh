@@ -28,8 +28,20 @@
 
 namespace zb {
 
-struct CParams { u32 windowLog, chainLog, hashLog, searchLog, minMatch, targetLength, strategy; };
+struct CParams {
+    u32 windowLog, chainLog, hashLog, searchLog, minMatch, targetLength, strategy;
+    ZB_HD bool any_set() const { return (windowLog | chainLog | hashLog | searchLog | minMatch | targetLength | strategy) != 0; }      // as overrides (0 = from the level)
+};
 enum : u32 { S_fast = 1, S_dfast = 2, S_greedy = 3, S_lazy = 4, S_lazy2 = 5, S_btlazy2 = 6 };
+
+// The explicit compression parameters in the order of ZSTD_c_windowLog (101) ... ZSTD_c_strategy (107): option name of
+// zstdb200_set_option, field, and the bounds of ZSTD_cParam_getBounds (N/compress/zstd_compress.c:420-520); 0 is always accepted.
+struct CParamBound { const char* option; u32 CParams::*member; int lo, hi;
+                     bool accepts(long long v) const { return v == 0 || (v >= lo && v <= hi); } };
+static const CParamBound CPARAM_BOUNDS[7] = {
+    { "c_windowLog", &CParams::windowLog, 10, 31 }, { "c_hashLog", &CParams::hashLog, 6, 30 }, { "c_chainLog", &CParams::chainLog, 6, 30 },
+    { "c_searchLog", &CParams::searchLog, 1, 30 }, { "c_minMatch", &CParams::minMatch, 3, 7 }, { "c_targetLength", &CParams::targetLength, 0, 131072 },
+    { "c_strategy", &CParams::strategy, 1, 9 } };
 
 constexpr u32 MAX_SEQ = (BLOCKSIZE_MAX / 4) + 8;
 constexpr u32 PARSE_SKIPPED = 0xFFFFFFFFu;     // nbSeq marker: srcSize < 7, the block is stored raw (ZSTD_buildSeqStore :3273-3280)
