@@ -102,8 +102,12 @@ ZSTDB200_API ZSTD_frameProgression ZSTD_getFrameProgression(const ZSTD_CCtx* cct
  * Compression scope of this build: srcSize <= 128 KB per call (one block => one frame), levels whose
  * parameters select the fast / dfast parsers, greedy / lazy / lazy2 (row-based match finder for inputs > 16 KB,
  * hash chain below) or btlazy2 (binary tree): the negative levels and levels 1..12 for srcSize > 16 KB, 1..10 for
- * srcSize <= 16 KB; the optimal-parser strategies above return
- * ZSTD_error_parameter_unsupported rather than silently producing different bytes.
+ * srcSize <= 16 KB; and the optimal parser (btopt / btultra / btultra2, levels 13..22 or ZSTD_c_strategy 7..9) for
+ * srcSize <= 64 KB.  Three cases return ZSTD_error_parameter_unsupported rather than different bytes: levels 11 and 12
+ * on srcSize <= 16 KB (btopt rows), the optimal parser on srcSize > 64 KB (the reference splits such blocks after
+ * the parse), and optimal levels in zstdb200_generate_sequences / zstdb200_sequenceProducer.  The batch calls, the
+ * begin/end pair, zstdb200_compress_device and the streams apply the rule per frame: at level 19 a stream fails on its
+ * first full 128 KB block, one shorter than 64 KB succeeds.
  * Decompression accepts any zstd stream without dictionary (multi-block, multi-frame, skippable, checksum). */
 ZSTDB200_API size_t ZSTD_compress2(ZSTD_CCtx* cctx, void* dst, size_t dstCapacity, const void* src, size_t srcSize);
 ZSTDB200_API size_t ZSTD_compress(void* dst, size_t dstCapacity, const void* src, size_t srcSize, int compressionLevel);

@@ -1,8 +1,10 @@
-"""Encoder fuzz (dev container: needs oracle/_ref): kernel source on the host / emulated warp vs the compiled reference on generated inputs of many shapes, levels and frame flags.  usage: python scripts/fuzz_encoder_vs_ref.py <seed> <seconds> [emu]"""
+"""Encoder fuzz (dev container: needs oracle/_ref): kernel source on the host / emulated warp vs the compiled reference on generated inputs of many shapes, levels and frame flags.  usage: python scripts/fuzz_encoder_vs_ref.py <seed> <seconds> [emu]
+Levels 13..22 (optimal parser) run on the first 64 KB of the input, through tests/hostsim/libzb_hostsim_opt.so."""
 import sys, random, time
 sys.path.insert(0, __import__('os').path.dirname(__import__('os').path.dirname(__import__('os').path.abspath(__file__))))
 import numpy as np
 from tests.oracle_util import *
+from tests.test_opt_levels import host as opt_compress
 seed=int(sys.argv[1]); T=float(sys.argv[2]); emu=len(sys.argv)>3
 rnd=random.Random(seed); rng=np.random.default_rng(seed)
 def gen():
@@ -34,11 +36,13 @@ def gen():
     return a.tobytes()
 t0=time.time(); n=0; bad=0
 while time.time()-t0<T:
-    d=gen(); lvl=rnd.choice([1,2,3,3,3,4,5,6,7,8,9,10,11,12,-1,-5,-50])
-    if len(d)<=16384 and lvl>10: continue
+    d=gen(); lvl=rnd.choice([1,2,3,3,3,4,5,6,7,8,9,10,11,12,-1,-5,-50]+list(range(13,23)))
+    if lvl>=13: d=d[:65536]
+    if len(d)<=16384 and lvl in (11,12): continue
     ck=rnd.random()<0.2; cs=rnd.random()<0.8
     e=ref_compress_flags(d,lvl,ck,cs,False)
-    if emu and lvl in (1,2,3,4,-1,-5,-50,5,6,7,8,9,10) and not ck and cs: g=emu_compress(d,lvl)
+    if lvl>=13: g=opt_compress(d,lvl,flags={"checksum":ck,"content_size":cs},emu=emu and rnd.random()<0.3)
+    elif emu and lvl in (1,2,3,4,-1,-5,-50,5,6,7,8,9,10) and not ck and cs: g=emu_compress(d,lvl)
     else: g=hostsim_compress_flags(d,lvl,ck,cs)
     n+=1
     if e!=g:

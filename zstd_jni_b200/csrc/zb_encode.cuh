@@ -1,14 +1,15 @@
 // zb_encode.cuh -- warp-cooperative one-shot Zstandard frame encoder for inputs of at
 // most one block (<= 128 KB): the unit of work of the batch API.  The emitted frame is
 // byte-identical to the reference's ZSTD_compress2(chunk, level) for the negative levels and
-// levels 1..12 (1..10 on inputs <= 16 KB), i.e. every strategy below the optimal parser.
+// levels 1..12 (1..10 on inputs <= 16 KB), and for the optimal-parser levels 13..22 on inputs <= 64 KB.
 //
 // Reference decisions being reproduced (N/ = luben/zstd-jni src/main/native/):
 //   parameters     N/compress/clevels.h:78-130, N/compress/zstd_compress.c:1472-1609,7759-7782
 //   framing        N/compress/zstd_compress.c:4591-4743,5344-5381
 //   parsers        N/compress/zstd_double_fast.c:105-323 (dfast), N/compress/zstd_fast.c:190-423 (fast),
 //                  N/compress/zstd_lazy.c:1516-1779 (greedy/lazy/lazy2/btlazy2) with the row-based (:775-1283),
-//                  hash-chain (:620-733) and binary-tree (:22-408) match finders
+//                  hash-chain (:620-733) and binary-tree (:22-408) match finders; N/compress/zstd_opt.c:45-1545 (btopt /
+//                  btultra / btultra2, one block, no dictionary)
 //   literals       N/compress/zstd_compress_literals.c:129-235, N/compress/huf_compress.c:146-1434, N/compress/hist.c
 //   sequences      N/compress/zstd_compress.c:2693-3042, N/compress/zstd_compress_sequences.c:17-382,
 //                  N/compress/fse_compress.c:68-525
@@ -32,7 +33,7 @@ struct CParams {
     u32 windowLog, chainLog, hashLog, searchLog, minMatch, targetLength, strategy;
     ZB_HD bool any_set() const { return (windowLog | chainLog | hashLog | searchLog | minMatch | targetLength | strategy) != 0; }      // as overrides (0 = from the level)
 };
-enum : u32 { S_fast = 1, S_dfast = 2, S_greedy = 3, S_lazy = 4, S_lazy2 = 5, S_btlazy2 = 6 };
+enum : u32 { S_fast = 1, S_dfast = 2, S_greedy = 3, S_lazy = 4, S_lazy2 = 5, S_btlazy2 = 6, S_btopt = 7, S_btultra = 8, S_btultra2 = 9 };
 
 // The explicit compression parameters in the order of ZSTD_c_windowLog (101) ... ZSTD_c_strategy (107): option name of
 // zstdb200_set_option, field, and the bounds of ZSTD_cParam_getBounds (N/compress/zstd_compress.c:420-520); 0 is always accepted.
@@ -46,17 +47,28 @@ static const CParamBound CPARAM_BOUNDS[7] = {
 constexpr u32 MAX_SEQ = (BLOCKSIZE_MAX / 4) + 8;
 constexpr u32 PARSE_SKIPPED = 0xFFFFFFFFu;     // nbSeq marker: srcSize < 7, the block is stored raw (ZSTD_buildSeqStore :3273-3280)
 constexpr u32 ENC_HASHLOG_MAX = 18;     // largest hashLog / chainLog of the supported rows
+// The optimal parser (btopt, btultra, btultra2) is served while the adjusted windowLog is at most 16, i.e. for inputs of at
+// most 64 KB: from windowLog 17 on the reference splits the block after the parse (ZSTD_resolveBlockSplitterMode,
+// N/compress/zstd_compress.c:248-252), which is not restated here.
+constexpr size_t OPT_SRC_MAX = 64 * 1024;
+constexpr u32 OPT_WINDOWLOG_MAX = 16;
 
 // ZSTD_getCParams_internal (:7759-7782) + ZSTD_adjustCParams_internal (:1472-1609) for a known
-// srcSize <= 128 KB, no dictionary.  Returns false when the level selects a parser this build lacks.
-// Level tables (clevels.h:78-92,104-116) in constant memory on the device, as a plain static on the host.
-struct LevelTables { CParams t128[13]; CParams t16[11]; };
+// srcSize <= 128 KB, no dictionary.  Returns false when the parameter set is outside what this build restates.
+// Level tables (clevels.h:78-130, rows 0..22) in constant memory on the device, as a plain static on the host.
+struct LevelTables { CParams t128[23]; CParams t16[23]; };
 #define ZB_LEVEL_TABLES_INIT { { {17,12,12,1,5,1,S_fast}, {17,12,13,1,6,0,S_fast}, {17,13,15,1,5,0,S_fast}, {17,15,16,2,5,0,S_dfast}, {17,17,17,2,4,0,S_dfast}, \
                                {17,16,17,3,4,2,S_greedy}, {17,16,17,3,4,4,S_lazy}, {17,16,17,3,4,8,S_lazy2}, {17,16,17,4,4,8,S_lazy2}, {17,16,17,5,4,8,S_lazy2}, \
-                               {17,16,17,6,4,8,S_lazy2}, {17,17,17,5,4,8,S_btlazy2}, {17,18,17,7,4,12,S_btlazy2} }, \
-                               { {14,12,13,1,5,1,S_fast}, {14,14,15,1,5,0,S_fast}, {14,14,15,1,4,0,S_fast}, {14,14,15,2,4,0,S_dfast}, \
-                             {14,14,14,4,4,2,S_greedy}, {14,14,14,3,4,4,S_lazy}, {14,14,14,4,4,8,S_lazy2}, {14,14,14,6,4,8,S_lazy2}, {14,14,14,8,4,8,S_lazy2}, \
-                              {14,15,14,5,4,8,S_btlazy2}, {14,15,14,9,4,8,S_btlazy2} } }
+                               {17,16,17,6,4,8,S_lazy2}, {17,17,17,5,4,8,S_btlazy2}, {17,18,17,7,4,12,S_btlazy2}, \
+                               {17,18,17,3,4,12,S_btopt}, {17,18,17,4,3,32,S_btopt}, {17,18,17,6,3,256,S_btopt}, {17,18,17,6,3,128,S_btultra}, \
+                               {17,18,17,8,3,256,S_btultra}, {17,18,17,10,3,512,S_btultra}, {17,18,17,5,3,256,S_btultra2}, {17,18,17,7,3,512,S_btultra2}, \
+                               {17,18,17,9,3,512,S_btultra2}, {17,18,17,11,3,999,S_btultra2} }, \
+                             { {14,12,13,1,5,1,S_fast}, {14,14,15,1,5,0,S_fast}, {14,14,15,1,4,0,S_fast}, {14,14,15,2,4,0,S_dfast}, \
+                               {14,14,14,4,4,2,S_greedy}, {14,14,14,3,4,4,S_lazy}, {14,14,14,4,4,8,S_lazy2}, {14,14,14,6,4,8,S_lazy2}, {14,14,14,8,4,8,S_lazy2}, \
+                               {14,15,14,5,4,8,S_btlazy2}, {14,15,14,9,4,8,S_btlazy2}, \
+                               {14,15,14,3,4,12,S_btopt}, {14,15,14,4,3,24,S_btopt}, {14,15,14,5,3,32,S_btultra}, {14,15,15,6,3,64,S_btultra}, \
+                               {14,15,15,7,3,256,S_btultra}, {14,15,15,5,3,48,S_btultra2}, {14,15,15,6,3,128,S_btultra2}, {14,15,15,7,3,256,S_btultra2}, \
+                               {14,15,15,8,3,256,S_btultra2}, {14,15,15,8,3,512,S_btultra2}, {14,15,15,9,3,512,S_btultra2}, {14,15,15,10,3,999,S_btultra2} } }
 #if defined(__CUDACC__)
 static __constant__ LevelTables c_levels = ZB_LEVEL_TABLES_INIT;
 #endif
@@ -84,16 +96,18 @@ ZB_HD void adjust_cparams(CParams& cp, size_t srcSize) {
 // checkWindow: refuse parameter sets whose window does not cover the input (matches would have to respect a sliding
 // window inside the block, which these parsers do not implement).
 ZB_HDN bool get_cparams(CParams* out, int level, size_t srcSize, const CParams* ov = nullptr, bool checkWindow = true) {
-    // rows 0..12 of the "<=128 KB" table and 0..10 of the "<=16 KB" table (clevels.h:78-92,104-116).  greedy / lazy / lazy2
-    // run with the row-based match finder when windowLog > 14 (ZSTD_resolveRowMatchFinderMode, zstd_compress.c:238-245),
-    // i.e. for every srcSize > 16 KB, and with the hash-chain finder below; btlazy2 uses the binary tree.  The rows from
-    // btopt on (optimal parser) are not built.
+    // rows 0..22 of the "<=128 KB" and "<=16 KB" tables (clevels.h:78-130).  greedy / lazy / lazy2 run with the row-based
+    // match finder when windowLog > 14 (ZSTD_resolveRowMatchFinderMode, zstd_compress.c:238-245), i.e. for every
+    // srcSize > 16 KB, and with the hash-chain finder below; btlazy2 uses the binary tree; btopt and up the optimal parser.
+    // Rows 11 and 12 of the "<=16 KB" table (btopt) stay refused, and so does every optimal-parser parameter set whose
+    // adjusted windowLog exceeds OPT_WINDOWLOG_MAX.
     if (srcSize > BLOCKSIZE_MAX) return false;
     int row = level;
     if (level == 0) row = 3;
     if (level < 0) row = 0;
+    if (row > 22) row = 22;
     bool const small = srcSize <= 16 * 1024;
-    if (row > (small ? 10 : 12)) return false;
+    if (small && (row == 11 || row == 12)) return false;
     CParams cp = small ? ZB_LEVELS.t16[row] : ZB_LEVELS.t128[row];
     if (level < 0) { int const l = level < -(1 << 17) ? -(1 << 17) : level; cp.targetLength = (u32)(-l); }
     adjust_cparams(cp, srcSize);
@@ -105,12 +119,24 @@ ZB_HDN bool get_cparams(CParams* out, int level, size_t srcSize, const CParams* 
         if (ov->minMatch) cp.minMatch = ov->minMatch;
         if (ov->targetLength) cp.targetLength = ov->targetLength;
         if (ov->strategy) cp.strategy = ov->strategy;
-        if (cp.strategy > S_btlazy2) return false;
         adjust_cparams(cp, srcSize);
         if (checkWindow && ((size_t)1 << cp.windowLog) < srcSize) return false;
     }
+    if (cp.strategy >= S_btopt && cp.windowLog > OPT_WINDOWLOG_MAX) return false;
     *out = cp;
     return true;
+}
+
+// Whether a level (explicit parameters: as get_cparams with checkWindow off) is served for some input of at most one block:
+// the entry points refuse the others before anything is launched.
+ZB_HDN bool level_served(int level, const CParams* ov = nullptr) {
+    CParams cp;
+    if (get_cparams(&cp, level, BLOCKSIZE_MAX, ov, false)) return true;
+    return get_cparams(&cp, level, OPT_SRC_MAX, ov, false) && cp.strategy >= S_btopt;
+}
+ZB_HDN bool level_is_optimal(int level, const CParams* ov = nullptr) {
+    CParams cp;
+    return get_cparams(&cp, level, OPT_SRC_MAX, ov, false) && cp.strategy >= S_btopt;
 }
 
 ZB_HD size_t compress_bound(size_t n) { return n + (n >> 8) + (n < (128u << 10) ? (((128u << 10) - n) >> 11) : 0); }
@@ -129,6 +155,10 @@ struct EncWork {
     u8* lit;            // BLOCKSIZE_MAX + 32
     u8* codes;          // 3 * MAX_SEQ
     u16* stbits;        // 3 * MAX_SEQ : per sequence and stream, FSE state bits (value | nbBits << 12)
+    struct OptNode* opt = nullptr;          // optimal parser only (enc_opt_work_carve): OPT_NUM + 3 nodes
+    struct OptMatch* matches = nullptr;     // OPT_NUM + 3 candidates of one position
+    u32* hash3 = nullptr;                   // 1 << OPT_WINDOWLOG_MAX entries
+    struct OptStats* stats = nullptr;       // symbol frequencies and base prices
 };
 ZB_HD size_t enc_entropy_work_bytes() { return (size_t)(BLOCKSIZE_MAX + 32) + 3 * (size_t)MAX_SEQ + 64 + 6 * (size_t)MAX_SEQ + 64; }
 ZB_HD void enc_entropy_work_carve(EncWork& w, u8* base) {
@@ -147,6 +177,28 @@ ZB_HD EncWork enc_work_carve(u8* base) {
     w.seq = reinterpret_cast<Seq*>(base); base += 16 * (size_t)MAX_SEQ;
     enc_entropy_work_carve(w, base);
     return w;
+}
+
+// ---- optimal parser state (ZSTD_optimal_t, ZSTD_match_t, optState_t of N/compress/zstd_compress_internal.h:160-240)
+constexpr u32 OPT_NUM = 1u << 12;          // ZSTD_OPT_NUM
+struct OptNode { int price; u32 off, mlen, litlen; u32 rep[3]; };
+struct OptMatch { u32 off, len; };
+struct OptStats {
+    u32 litFreq[256], llFreq[MaxLL + 1], mlFreq[MaxML + 1], ofFreq[MaxOff + 1];
+    u32 litSum, llSum, mlSum, ofSum;
+    u32 litSumBase, llSumBase, mlSumBase, ofSumBase;      // WEIGHT of the sums (ZSTD_setBasePrices)
+    u32 predef;                                           // zop_predef: static prices (first block of <= 8 bytes)
+};
+// Global workspace of one optimal-parser warp, allocated only when such a level is launched.
+ZB_HD size_t enc_opt_work_bytes() {
+    return (size_t)sizeof(OptNode) * (OPT_NUM + 3) + 16 + (size_t)sizeof(OptMatch) * (OPT_NUM + 3) + 16 + ((size_t)4 << OPT_WINDOWLOG_MAX) + sizeof(OptStats) + 64;
+}
+ZB_HD void enc_opt_work_carve(EncWork& w, u8* base) {
+    auto align16 = [](u8* p) { return reinterpret_cast<u8*>((reinterpret_cast<uintptr_t>(p) + 15) & ~(uintptr_t)15); };
+    base = align16(base); w.opt = reinterpret_cast<OptNode*>(base); base += sizeof(OptNode) * (OPT_NUM + 3);
+    base = align16(base); w.matches = reinterpret_cast<OptMatch*>(base); base += sizeof(OptMatch) * (OPT_NUM + 3);
+    base = align16(base); w.hash3 = reinterpret_cast<u32*>(base); base += (size_t)4 << OPT_WINDOWLOG_MAX;
+    w.stats = reinterpret_cast<OptStats*>(base);
 }
 
 // ---- per-warp shared scratch
@@ -998,6 +1050,31 @@ ZB_HDN size_t huf_encode_stream(const C& w, const EncShared& S, u8* dst, size_t 
     return size;
 }
 
+// HUF_optimalTableLog with HUF_flags_optimalDepth (huf_compress.c:1289-1326, strategy >= btultra): the table log from
+// HUF_minTableLog(cardinality) up that gives the smallest description + payload, stopping once the size grows.  The
+// descriptions are written to `dst` as scratch (the final one overwrites them).  Lane 0; S.count holds the histogram.
+ZB_HDN u32 huf_optimal_depth(EncShared& S, u8* dst, size_t cap, u32 maxSV, u32 maxTableLog) {
+    u32 cardinality = 0;
+    for (u32 s = 0; s <= maxSV; s++) cardinality += S.count[s] != 0;
+    u32 const minTableLog = highbit32(cardinality) + 1;
+    size_t optSize = ~(size_t)0 - 1;
+    u32 optLog = maxTableLog;
+    for (u32 guess = minTableLog; guess <= maxTableLog; guess++) {
+        u32 const maxBits = huf_build_ctable(S, S.count, maxSV, guess);
+        if (maxBits < guess && guess > minTableLog) break;
+        size_t const hSize = huf_write_ctable(S, dst, cap, maxSV, maxBits);
+        if (isErr(hSize)) continue;
+        size_t bits = 0;      // HUF_estimateCompressedSize
+        for (u32 s = 0; s <= maxSV; s++) bits += (size_t)S.hufBits[s] * S.count[s];
+        size_t const newSize = (bits >> 3) + hSize;
+        if (newSize > optSize + 1) break;
+        if (newSize < optSize) { optSize = newSize; optLog = guess; }
+    }
+    return optLog;
+}
+// ZSTD_minGain (zstd_compress_internal.h:677-682): the saving a compressed block or literals section must reach
+ZB_HD size_t min_gain(size_t n, u32 strategy) { u32 const minlog = strategy >= S_btultra ? strategy - 1 : 6; return (n >> minlog) + 2; }
+
 // ZSTD_noCompressLiterals :39-66 / ZSTD_compressRleLiteralsBlock :81-107 ; warp copy
 template <class C>
 ZB_HDN size_t lit_raw(const C& w, u8* dst, size_t cap, const u8* src, size_t n) {
@@ -1053,7 +1130,8 @@ ZB_HDN size_t compress_literals(const C& w, EncShared& S, u8* dst, size_t cap, c
         // tree + table description on lane 0
         size_t hSize = 0; u32 huffLog = 0;
         if (w.lane == 0) {
-            huffLog = fse_optimal_log(LitHufLog, n, maxSV, 1);     // HUF_optimalTableLog cheap path :1284-1287
+            huffLog = strategy >= S_btultra ? huf_optimal_depth(S, o, ocap, maxSV, LitHufLog)      // HUF_flags_optimalDepth
+                                            : fse_optimal_log(LitHufLog, n, maxSV, 1);             // HUF_optimalTableLog cheap path :1284-1287
             huffLog = huf_build_ctable(S, S.count, maxSV, huffLog);
             hSize = huf_write_ctable(S, o, ocap, maxSV, huffLog);
         }
@@ -1101,8 +1179,7 @@ ZB_HDN size_t compress_literals(const C& w, EncShared& S, u8* dst, size_t cap, c
     } while (0);
     w.sync();
     ZB_PT(9);          // Huffman streams
-    {   size_t const minGain = (n >> 6) + 2;
-        if (cLit == 0 || isErr(cLit) || cLit >= n - minGain) return lit_raw(w, dst, cap, src, n); }
+    if (cLit == 0 || isErr(cLit) || cLit >= n - min_gain(n, strategy)) return lit_raw(w, dst, cap, src, n);
     if (cLit == 1) {
         // n >= 64 here, so the "single byte really is the whole literal run" check of :199-206 holds
         return lit_rle(w, dst, src, n);
@@ -2154,6 +2231,377 @@ ZB_HDN u32 parse_lazy_warp(const C& w, const EncWork& W, const u8* src, size_t s
 // every lane follows with shuffles (three registers), lane k keeping the offset of its own sequence.
 // A block the reference would not parse (srcSize < 7, PARSE_SKIPPED) is exported as literals only.  Returns the number
 // of records (uniform), at most MAX_SEQ + 1.
+// ------------------------------------------------------------------ optimal parser (btopt / btultra / btultra2)
+// N/compress/zstd_opt.c for one block, no dictionary, no LDM: prices (:45-391), hash3 (:409-430), binary tree (:440-585),
+// match gathering (:587-850), the forward/backward parse (:1074-1442), btultra2's statistics pass (:1482-1543).  Serial: lane 0
+// runs it.  Indices are the reference's: position p of the block has index p + B, with B = 2 (ZSTD_WINDOW_START_INDEX) and,
+// in btultra2's second pass, B = 2 + srcSize (the first pass is moved out of the window, `base -= srcSize`).
+constexpr u32 OPT_MAX_PRICE = 1u << 30, OPT_PREDEF_THRESHOLD = 8, OPT_LITFREQ_ADD = 2;
+ZB_HD u32 opt_weight(u32 stat, int optLevel) {      // ZSTD_bitWeight / ZSTD_fracWeight, BITCOST_ACCURACY 8
+    if (!optLevel) return highbit32(stat + 1) * 256;
+    u32 const s = stat + 1, hb = highbit32(s);
+    return hb * 256 + ((s << 8) >> hb);
+}
+ZB_HD u32 opt_downscale(u32* t, u32 last, u32 shift, bool base1) {
+    u32 sum = 0;
+    for (u32 s = 0; s <= last; s++) { u32 const v = (base1 ? 1u : (t[s] > 0)) + (t[s] >> shift); sum += v; t[s] = v; }
+    return sum;
+}
+ZB_HD u32 opt_scale(u32* t, u32 last, u32 logTarget) {
+    u32 prev = 0;
+    for (u32 s = 0; s <= last; s++) prev += t[s];
+    u32 const factor = prev >> logTarget;
+    if (factor <= 1) return prev;
+    return opt_downscale(t, last, highbit32(factor), true);
+}
+ZB_HD void opt_base_prices(OptStats& st, int optLevel) {
+    st.litSumBase = opt_weight(st.litSum, optLevel); st.llSumBase = opt_weight(st.llSum, optLevel);
+    st.mlSumBase = opt_weight(st.mlSum, optLevel); st.ofSumBase = opt_weight(st.ofSum, optLevel);
+}
+// ZSTD_rescaleFreqs: the first call of a frame starts from the literal histogram of the block and fixed sequence frequencies;
+// a later call (btultra2's second pass) scales the collected statistics down
+ZB_HDN void opt_rescale(OptStats& st, const u8* src, u32 srcSize, int optLevel) {
+    st.predef = 0;
+    if (st.llSum == 0) {
+        if (srcSize <= OPT_PREDEF_THRESHOLD) st.predef = 1;
+        for (u32 s = 0; s < 256; s++) st.litFreq[s] = 0;
+        for (u32 i = 0; i < srcSize; i++) st.litFreq[src[i]]++;
+        st.litSum = opt_downscale(st.litFreq, 255, 8, false);
+        // baseLLfreqs {4, 2, 1, ...} and baseOFCfreqs {6, 2, 1, 1, 2, 3, 4, 4, 4, 3, 2, 1, ...}
+        st.llSum = 0;
+        for (u32 s = 0; s <= MaxLL; s++) { u32 const f = s == 0 ? 4 : s == 1 ? 2 : 1; st.llFreq[s] = f; st.llSum += f; }
+        for (u32 s = 0; s <= MaxML; s++) st.mlFreq[s] = 1;
+        st.mlSum = MaxML + 1;
+        st.ofSum = 0;
+        for (u32 s = 0; s <= MaxOff; s++) { u32 const f = s < 11 ? (u32)(0x62112344432ull >> (4 * (10 - s))) & 15 : 1; st.ofFreq[s] = f; st.ofSum += f; }
+    } else {
+        st.litSum = opt_scale(st.litFreq, 255, 12);
+        st.llSum = opt_scale(st.llFreq, MaxLL, 11);
+        st.mlSum = opt_scale(st.mlFreq, MaxML, 11);
+        st.ofSum = opt_scale(st.ofFreq, MaxOff, 11);
+    }
+    opt_base_prices(st, optLevel);
+}
+ZB_HD u32 opt_lit_price(const OptStats& st, u8 c, int optLevel) {      // ZSTD_rawLiteralsCost of one literal
+    if (st.predef) return 6 * 256;
+    u32 const maxP = st.litSumBase - 256;
+    u32 p = opt_weight(st.litFreq[c], optLevel);
+    if (p > maxP) p = maxP;
+    return st.litSumBase - p;
+}
+ZB_HD u32 opt_ll_price(const OptStats& st, u32 ll, int optLevel) {     // ZSTD_litLengthPrice (ll < BLOCKSIZE_MAX here)
+    if (st.predef) return opt_weight(ll, optLevel);
+    u32 const c = ll_code(ll);
+    return (u32)ZB_T.LL_bits[c] * 256 + st.llSumBase - opt_weight(st.llFreq[c], optLevel);
+}
+ZB_HD u32 opt_match_price(const OptStats& st, u32 offBase, u32 ml, int optLevel) {      // ZSTD_getMatchPrice
+    u32 const offCode = highbit32(offBase), mlBase = ml - MINMATCH;
+    if (st.predef) return opt_weight(mlBase, optLevel) + (16 + offCode) * 256;
+    u32 price = offCode * 256 + (st.ofSumBase - opt_weight(st.ofFreq[offCode], optLevel));
+    if (optLevel < 2 && offCode >= 20) price += (offCode - 19) * 2 * 256;
+    u32 const mlCode = ml_code(mlBase);
+    price += (u32)ZB_T.ML_bits[mlCode] * 256 + (st.mlSumBase - opt_weight(st.mlFreq[mlCode], optLevel));
+    return price + 256 / 5;
+}
+ZB_HD void opt_update_stats(OptStats& st, u32 ll, const u8* lit, u32 offBase, u32 ml) {
+    for (u32 u = 0; u < ll; u++) st.litFreq[lit[u]] += OPT_LITFREQ_ADD;
+    st.litSum += ll * OPT_LITFREQ_ADD;
+    st.llFreq[ll_code(ll)]++; st.llSum++;
+    st.ofFreq[highbit32(offBase)]++; st.ofSum++;
+    st.mlFreq[ml_code(ml - MINMATCH)]++; st.mlSum++;
+}
+ZB_HD void opt_new_rep(u32* r, const u32* prev, u32 offBase, u32 ll0) {      // ZSTD_newRep / ZSTD_updateRep
+    r[0] = prev[0]; r[1] = prev[1]; r[2] = prev[2];
+    if (offBase > 3) { r[2] = r[1]; r[1] = r[0]; r[0] = offBase - 3; return; }
+    u32 const repCode = offBase - 1 + ll0;
+    if (repCode > 0) {
+        u32 const cur = (repCode == 3) ? r[0] - 1 : r[repCode];
+        r[2] = (repCode >= 2) ? r[1] : r[2];
+        r[1] = r[0]; r[0] = cur;
+    }
+}
+
+struct OptMs {
+    const u8* src; u32 srcSize, B;          // block, index of its first byte (= dictLimit = lowLimit)
+    u32* hashTable; u32* bt; u32* hash3;
+    u32 hashLog, btMask, searchLog, mls, hashLog3, nextToUpdate, targetLength;
+    ZB_HD const u8* at(u32 idx) const { return src + (idx - B); }
+};
+ZB_HD u32 opt_hash3(const u8* p, u32 h) { return ((load32(p) << 8) * 506832829u) >> (32 - h); }
+ZB_HD u32 opt_read_min(const u8* p, u32 mm) { return mm == 3 ? load32(p) << 8 : load32(p); }      // ZSTD_readMINMATCH
+
+// ZSTD_insertBt1: inserts index `curr` into the tree; returns how many positions the caller may advance
+ZB_HDN u32 opt_insert_bt1(OptMs& ms, u32 curr) {
+    const u8* const ip = ms.at(curr); const u8* const iend = ms.src + ms.srcSize;
+    u32 const h = hash_ptr(ip, ms.hashLog, ms.mls);
+    u32 matchIndex = ms.hashTable[h];
+    size_t commonLengthSmaller = 0, commonLengthLarger = 0;
+    u32 const btLow = ms.btMask >= curr ? 0 : curr - ms.btMask;
+    u32* smallerPtr = ms.bt + 2 * (curr & ms.btMask);
+    u32* largerPtr = smallerPtr + 1;
+    u32 dummy32;
+    u32 const windowLow = ms.B;
+    u32 matchEndIdx = curr + 8 + 1;
+    size_t bestLength = 8;
+    u32 nbCompares = 1u << ms.searchLog;
+    ms.hashTable[h] = curr;
+    for (; nbCompares && (matchIndex >= windowLow); --nbCompares) {
+        u32* const nextPtr = ms.bt + 2 * (matchIndex & ms.btMask);
+        size_t matchLength = commonLengthSmaller < commonLengthLarger ? commonLengthSmaller : commonLengthLarger;
+        const u8* const match = ms.at(matchIndex);
+        matchLength += count_match(ip + matchLength, match + matchLength, iend);
+        if (matchLength > bestLength) {
+            bestLength = matchLength;
+            if (matchLength > matchEndIdx - matchIndex) matchEndIdx = matchIndex + (u32)matchLength;
+        }
+        if (ip + matchLength == iend) break;
+        if (match[matchLength] < ip[matchLength]) {
+            *smallerPtr = matchIndex; commonLengthSmaller = matchLength;
+            if (matchIndex <= btLow) { smallerPtr = &dummy32; break; }
+            smallerPtr = nextPtr + 1; matchIndex = nextPtr[1];
+        } else {
+            *largerPtr = matchIndex; commonLengthLarger = matchLength;
+            if (matchIndex <= btLow) { largerPtr = &dummy32; break; }
+            largerPtr = nextPtr; matchIndex = nextPtr[0];
+        }
+    }
+    *smallerPtr = *largerPtr = 0;
+    u32 positions = 0;
+    if (bestLength > 384) positions = (bestLength - 384) < 192 ? (u32)(bestLength - 384) : 192u;
+    u32 const fwd = matchEndIdx - (curr + 8);
+    return positions > fwd ? positions : fwd;
+}
+
+// ZSTD_btGetAllMatches_internal (noDict) = ZSTD_updateTree + ZSTD_insertBtAndGetAllMatches: the candidates of position `curr`
+// by increasing length (repcodes, then the hash3 match, then the tree), each longer than the previous
+ZB_HDN u32 opt_get_all_matches(OptMs& ms, OptMatch* matches, u32* nextToUpdate3, u32 curr, const u32* rep, u32 ll0, u32 lengthToBeat) {
+    if (curr < ms.nextToUpdate) return 0;      // skipped area
+    for (u32 idx = ms.nextToUpdate; idx < curr;) idx += opt_insert_bt1(ms, idx);
+    ms.nextToUpdate = curr;
+    const u8* const ip = ms.at(curr); const u8* const iLimit = ms.src + ms.srcSize;
+    u32 const sufficient_len = ms.targetLength < OPT_NUM - 1 ? ms.targetLength : OPT_NUM - 1;
+    u32 const minMatch = (ms.mls == 3) ? 3 : 4;
+    u32 const h = hash_ptr(ip, ms.hashLog, ms.mls);
+    u32 matchIndex = ms.hashTable[h];
+    size_t commonLengthSmaller = 0, commonLengthLarger = 0;
+    u32 const dictLimit = ms.B, windowLow = ms.B, matchLow = windowLow ? windowLow : 1;
+    u32 const btLow = (ms.btMask >= curr) ? 0 : curr - ms.btMask;
+    u32* smallerPtr = ms.bt + 2 * (curr & ms.btMask);
+    u32* largerPtr = smallerPtr + 1;
+    u32 matchEndIdx = curr + 8 + 1;
+    u32 dummy32;
+    u32 mnum = 0;
+    u32 nbCompares = 1u << ms.searchLog;
+    size_t bestLength = lengthToBeat - 1;
+    {   u32 const lastR = 3 + ll0;
+        for (u32 repCode = ll0; repCode < lastR; repCode++) {
+            u32 const repOffset = (repCode == 3) ? (rep[0] - 1) : rep[repCode];
+            u32 const repIndex = curr - repOffset;
+            u32 repLen = 0;
+            if (repOffset - 1 < curr - dictLimit) {
+                if ((repIndex >= windowLow) && (opt_read_min(ip, minMatch) == opt_read_min(ip - repOffset, minMatch)))
+                    repLen = count_match(ip + minMatch, ip + minMatch - repOffset, iLimit) + minMatch;
+            }
+            if (repLen > bestLength) {
+                bestLength = repLen;
+                matches[mnum].off = repCode - ll0 + 1; matches[mnum].len = repLen; mnum++;
+                if ((repLen > sufficient_len) || (ip + repLen == iLimit)) return mnum;
+            }
+        } }
+    if (ms.mls == 3 && bestLength < 3) {      // HC3 match finder (ZSTD_insertAndFindFirstIndexHash3)
+        for (u32 idx = *nextToUpdate3; idx < curr; idx++) ms.hash3[opt_hash3(ms.at(idx), ms.hashLog3)] = idx;
+        *nextToUpdate3 = curr;
+        u32 const matchIndex3 = ms.hash3[opt_hash3(ip, ms.hashLog3)];
+        if ((matchIndex3 >= matchLow) && (curr - matchIndex3 < (1u << 18))) {
+            size_t const mlen = count_match(ip, ms.at(matchIndex3), iLimit);
+            if (mlen >= 3) {
+                bestLength = mlen;
+                matches[0].off = curr - matchIndex3 + 3; matches[0].len = (u32)mlen; mnum = 1;
+                if ((mlen > sufficient_len) || (ip + mlen == iLimit)) { ms.nextToUpdate = curr + 1; return 1; }
+            }
+        }
+    }
+    ms.hashTable[h] = curr;
+    for (; nbCompares && (matchIndex >= matchLow); --nbCompares) {
+        u32* const nextPtr = ms.bt + 2 * (matchIndex & ms.btMask);
+        size_t matchLength = commonLengthSmaller < commonLengthLarger ? commonLengthSmaller : commonLengthLarger;
+        const u8* const match = ms.at(matchIndex);
+        matchLength += count_match(ip + matchLength, match + matchLength, iLimit);
+        if (matchLength > bestLength) {
+            if (matchLength > matchEndIdx - matchIndex) matchEndIdx = matchIndex + (u32)matchLength;
+            bestLength = matchLength;
+            matches[mnum].off = curr - matchIndex + 3; matches[mnum].len = (u32)matchLength; mnum++;
+            if ((matchLength > OPT_NUM) || (ip + matchLength == iLimit)) break;
+        }
+        if (match[matchLength] < ip[matchLength]) {
+            *smallerPtr = matchIndex; commonLengthSmaller = matchLength;
+            if (matchIndex <= btLow) { smallerPtr = &dummy32; break; }
+            smallerPtr = nextPtr + 1; matchIndex = nextPtr[1];
+        } else {
+            *largerPtr = matchIndex; commonLengthLarger = matchLength;
+            if (matchIndex <= btLow) { largerPtr = &dummy32; break; }
+            largerPtr = nextPtr; matchIndex = nextPtr[0];
+        }
+    }
+    *smallerPtr = *largerPtr = 0;
+    ms.nextToUpdate = matchEndIdx - 8;
+    return mnum;
+}
+
+// ZSTD_compressBlock_opt_generic (noDict): sequences into W.seq from *nbSeq on, the repcode history in rep[];
+// returns the trailing literal count
+ZB_HDN u32 opt_block(OptMs& ms, const EncWork& W, u32* rep, int optLevel, u32* nbSeq) {
+    OptStats& st = *W.stats;
+    OptNode* const opt = W.opt;
+    OptMatch* const matches = W.matches;
+    const u8* const src = ms.src; u32 const srcSize = ms.srcSize;
+    u32 const sufficient_len = ms.targetLength < OPT_NUM - 1 ? ms.targetLength : OPT_NUM - 1;
+    u32 const minMatch = (ms.mls == 3) ? 3 : 4;
+    u32 nextToUpdate3 = ms.nextToUpdate;
+    OptNode lastStretch; lastStretch.price = 0; lastStretch.off = 0; lastStretch.mlen = 0; lastStretch.litlen = 0; lastStretch.rep[0] = lastStretch.rep[1] = lastStretch.rep[2] = 0;
+    opt_rescale(st, src, srcSize, optLevel);
+    auto LL_PRICE = [&](u32 l) { return (int)opt_ll_price(st, l, optLevel); };
+    auto LIT_PRICE = [&](u32 p) { return (int)opt_lit_price(st, src[p], optLevel); };
+    u32 ip = 1, anchor = 0;      // positions in the block (ip += (ip == prefixStart))
+    while (ip + 8 < srcSize) {   // ip < ilimit = iend - 8
+        u32 cur, last_pos = 0;
+        {   u32 const litlen = ip - anchor, ll0 = !litlen;
+            u32 const nbMatches = opt_get_all_matches(ms, matches, &nextToUpdate3, ip + ms.B, rep, ll0, minMatch);
+            if (!nbMatches) { ip++; continue; }
+            opt[0].mlen = 0; opt[0].litlen = litlen; opt[0].price = LL_PRICE(litlen);
+            opt[0].rep[0] = rep[0]; opt[0].rep[1] = rep[1]; opt[0].rep[2] = rep[2];
+            u32 const maxML = matches[nbMatches - 1].len, maxOffBase = matches[nbMatches - 1].off;
+            if (maxML > sufficient_len) {
+                lastStretch.litlen = 0; lastStretch.mlen = maxML; lastStretch.off = maxOffBase;
+                cur = 0; last_pos = maxML;
+                goto shortest_path;
+            }
+            u32 pos = 1;
+            for (; pos < minMatch; pos++) { opt[pos].price = (int)OPT_MAX_PRICE; opt[pos].mlen = 0; opt[pos].litlen = litlen + pos; }
+            for (u32 m = 0; m < nbMatches; m++) {
+                u32 const offBase = matches[m].off, end = matches[m].len;
+                for (; pos <= end; pos++) {
+                    int const sequencePrice = opt[0].price + (int)opt_match_price(st, offBase, pos, optLevel);
+                    opt[pos].mlen = pos; opt[pos].off = offBase; opt[pos].litlen = 0; opt[pos].price = sequencePrice + LL_PRICE(0);
+                }
+            }
+            last_pos = pos - 1;
+            opt[pos].price = (int)OPT_MAX_PRICE;
+        }
+        for (cur = 1; cur <= last_pos; cur++) {
+            u32 const inr = ip + cur;
+            {   u32 const litlen = opt[cur - 1].litlen + 1;
+                int const price = opt[cur - 1].price + LIT_PRICE(ip + cur - 1) + (LL_PRICE(litlen) - LL_PRICE(litlen - 1));
+                if (price <= opt[cur].price) {
+                    OptNode const prevMatch = opt[cur];
+                    opt[cur] = opt[cur - 1];
+                    opt[cur].litlen = litlen; opt[cur].price = price;
+                    if ((optLevel >= 1) && (prevMatch.litlen == 0) && (LL_PRICE(1) - LL_PRICE(0) < 0) && (ip + cur < srcSize)) {
+                        int const with1literal = prevMatch.price + LIT_PRICE(ip + cur) + (LL_PRICE(1) - LL_PRICE(0));
+                        int const withMoreLiterals = price + LIT_PRICE(ip + cur) + (LL_PRICE(litlen + 1) - LL_PRICE(litlen));
+                        if ((with1literal < withMoreLiterals) && (with1literal < opt[cur + 1].price)) {
+                            u32 const prev = cur - prevMatch.mlen;
+                            u32 newReps[3]; opt_new_rep(newReps, opt[prev].rep, prevMatch.off, opt[prev].litlen == 0);
+                            opt[cur + 1] = prevMatch;
+                            opt[cur + 1].rep[0] = newReps[0]; opt[cur + 1].rep[1] = newReps[1]; opt[cur + 1].rep[2] = newReps[2];
+                            opt[cur + 1].litlen = 1; opt[cur + 1].price = with1literal;
+                            if (last_pos < cur + 1) last_pos = cur + 1;
+                        }
+                    }
+                }
+            }
+            if (opt[cur].litlen == 0) {      // just finished a match: the offset history moves
+                u32 const prev = cur - opt[cur].mlen;
+                u32 newReps[3]; opt_new_rep(newReps, opt[prev].rep, opt[cur].off, opt[prev].litlen == 0);
+                opt[cur].rep[0] = newReps[0]; opt[cur].rep[1] = newReps[1]; opt[cur].rep[2] = newReps[2];
+            }
+            if (inr + 8 > srcSize) continue;      // inr > ilimit
+            if (cur == last_pos) break;
+            if ((optLevel == 0) && (opt[cur + 1].price <= opt[cur].price + 256 / 2)) continue;
+            {   u32 const ll0 = (opt[cur].litlen == 0);
+                int const basePrice = opt[cur].price + LL_PRICE(0);
+                u32 const nbMatches = opt_get_all_matches(ms, matches, &nextToUpdate3, inr + ms.B, opt[cur].rep, ll0, minMatch);
+                if (!nbMatches) continue;
+                {   u32 const longestML = matches[nbMatches - 1].len;
+                    if ((longestML > sufficient_len) || (cur + longestML >= OPT_NUM) || (ip + cur + longestML >= srcSize)) {
+                        lastStretch.mlen = longestML; lastStretch.off = matches[nbMatches - 1].off; lastStretch.litlen = 0;
+                        last_pos = cur + longestML;
+                        goto shortest_path;
+                    } }
+                for (u32 m = 0; m < nbMatches; m++) {
+                    u32 const offset = matches[m].off, lastML = matches[m].len;
+                    u32 const startML = (m > 0) ? matches[m - 1].len + 1 : minMatch;
+                    for (u32 mlen = lastML; mlen >= startML; mlen--) {      // scan downward
+                        u32 const pos = cur + mlen;
+                        int const price = basePrice + (int)opt_match_price(st, offset, mlen, optLevel);
+                        if ((pos > last_pos) || (price < opt[pos].price)) {
+                            while (last_pos < pos) { last_pos++; opt[last_pos].price = (int)OPT_MAX_PRICE; opt[last_pos].litlen = 1; }
+                            opt[pos].mlen = mlen; opt[pos].off = offset; opt[pos].litlen = 0; opt[pos].price = price;
+                        } else if (optLevel == 0) break;      // early abort
+                    }
+                }
+            }
+            opt[last_pos + 1].price = (int)OPT_MAX_PRICE;
+        }
+        lastStretch = opt[last_pos];
+        cur = last_pos - lastStretch.mlen;
+    shortest_path:
+        if (lastStretch.mlen == 0) { ip += last_pos; continue; }      // only literals
+        if (lastStretch.litlen == 0) { u32 r[3]; opt_new_rep(r, opt[cur].rep, lastStretch.off, opt[cur].litlen == 0); rep[0] = r[0]; rep[1] = r[1]; rep[2] = r[2]; }
+        else { rep[0] = lastStretch.rep[0]; rep[1] = lastStretch.rep[1]; rep[2] = lastStretch.rep[2]; cur -= lastStretch.litlen; }
+        {   u32 const storeEnd = cur + 2;
+            u32 storeStart = storeEnd, stretchPos = cur;
+            if (lastStretch.litlen > 0) {
+                opt[storeEnd].litlen = lastStretch.litlen; opt[storeEnd].mlen = 0;
+                opt[storeEnd - 1] = lastStretch;
+            }
+            opt[storeEnd] = lastStretch;
+            storeStart = storeEnd;
+            for (;;) {
+                OptNode const nextStretch = opt[stretchPos];
+                opt[storeStart].litlen = nextStretch.litlen;
+                if (nextStretch.mlen == 0) break;
+                storeStart--;
+                opt[storeStart] = nextStretch;
+                stretchPos -= nextStretch.litlen + nextStretch.mlen;
+            }
+            for (u32 sp = storeStart; sp <= storeEnd; sp++) {
+                u32 const llen = opt[sp].litlen, mlen = opt[sp].mlen, offBase = opt[sp].off;
+                if (mlen == 0) { ip = anchor + llen; continue; }
+                opt_update_stats(st, llen, src + anchor, offBase, mlen);
+                W.put(*nbSeq, llen, offBase, mlen); (*nbSeq)++;
+                anchor += llen + mlen;
+                ip = anchor;
+            }
+            opt_base_prices(st, optLevel);
+        }
+    }
+    return srcSize - anchor;
+}
+
+// One block with the optimal parser on a fresh frame.  Tables (hashTable = W.hashLong, tree = W.hashSmall, W.hash3) are zeroed by
+// the caller; strategy btultra2 first parses the block once to seed the statistics (ZSTD_initStats_ultra).
+ZB_HDN u32 parse_opt(const EncWork& W, const u8* src, size_t srcSize, const CParams& cp, u32* lastLL) {
+    OptMs ms;
+    ms.src = src; ms.srcSize = (u32)srcSize; ms.B = 2;
+    ms.hashTable = W.hashLong; ms.bt = W.hashSmall; ms.hash3 = W.hash3;
+    ms.hashLog = cp.hashLog; ms.btMask = (1u << (cp.chainLog - 1)) - 1; ms.searchLog = cp.searchLog;
+    ms.mls = cp.minMatch < 3 ? 3 : cp.minMatch > 6 ? 6 : cp.minMatch;
+    ms.hashLog3 = cp.minMatch == 3 ? (cp.windowLog < 17 ? cp.windowLog : 17) : 0;
+    ms.nextToUpdate = 2; ms.targetLength = cp.targetLength;
+    int const optLevel = cp.strategy == S_btopt ? 0 : 2;
+    W.stats->llSum = 0;      // first block: statistics start from the input
+    u32 rep[3] = { 1, 4, 8 }, nbSeq = 0;
+    if (cp.strategy == S_btultra2 && srcSize > OPT_PREDEF_THRESHOLD) {
+        u32 tmpRep[3] = { 1, 4, 8 };
+        (void)opt_block(ms, W, tmpRep, optLevel, &nbSeq);
+        nbSeq = 0;                                             // the first pass only leaves its statistics
+        ms.B += (u32)srcSize; ms.nextToUpdate = ms.B;          // base -= srcSize; dictLimit = lowLimit = nextToUpdate += srcSize
+    }
+    *lastLL = opt_block(ms, W, rep, optLevel, &nbSeq);
+    return nbSeq;
+}
+
 struct alignas(16) ZSeq { u32 offset, litLength, matchLength, rep; };
 template <class C>
 ZB_HDN u32 export_sequences(const C& w, const Seq* in, u32 nbSeq, u32 lastLL, size_t srcSize, ZSeq* out) {
@@ -2195,27 +2643,43 @@ constexpr u32 FRAME_CHECKSUM = 1, FRAME_NO_CONTENT_SIZE = 2, FRAME_MAGICLESS = 4
 // strategy for every input size, so the kernel holds a single cooperative parser (64 registers without spills; the
 // all-in-one instantiation needs ~1 KB of stack).  ONLY = ONLY_LAZY: greedy ... btlazy2 for every input size (levels 5 and up):
 // the cooperative row-based parser plus the serial finders, built with its own register budget.
-constexpr u32 ONLY_LAZY = 64;
+// ONLY = ONLY_OPT: the optimal parser alone (btopt ... btultra2, inputs <= OPT_SRC_MAX); it needs the workspace of
+// enc_opt_work_carve.  The device's all-in-one instantiation leaves it out; the host instantiations keep every parser.
+constexpr u32 ONLY_LAZY = 64, ONLY_OPT = 65;
 template <class C, u32 ONLY = 0>
 ZB_HDN size_t parse_stage(const C& w, const EncWork& W, const u8* src, size_t srcSize, int level, u32* nbSeqOut, u32* lastLLOut, const CParams* ov = nullptr) {
+#if defined(__CUDA_ARCH__)
+    constexpr bool withOpt = ONLY == ONLY_OPT;
+#else
+    constexpr bool withOpt = ONLY == ONLY_OPT || ONLY == 0;
+#endif
     CParams cp;
     *nbSeqOut = PARSE_SKIPPED; *lastLLOut = 0;
     if (!get_cparams(&cp, level, srcSize, ov)) return ERR(E_parameter_unsupported);
-    if (ONLY == ONLY_LAZY ? cp.strategy < S_greedy : (ONLY != 0 && cp.strategy != ONLY)) return ERR(E_GENERIC);
+    {   bool const fits = ONLY == ONLY_OPT ? cp.strategy >= S_btopt
+                        : ONLY == ONLY_LAZY ? (cp.strategy >= S_greedy && cp.strategy <= S_btlazy2)
+                        : ONLY != 0 ? cp.strategy == ONLY : (cp.strategy < S_btopt || withOpt);
+        if (!fits || (cp.strategy >= S_btopt && !W.opt)) return ERR(E_GENERIC); }
     if (srcSize < 7) return 0;
     {   // fresh tables: zero the used part (16-byte stores; the workspace is 16-byte aligned)
         u32 const nL = (1u << cp.hashLog) / 4;
         u32 const nS = (cp.strategy == S_dfast) ? (1u << cp.chainLog) / 4                               // short-hash table
-                     : (cp.strategy >= S_greedy) ? ((cp.strategy != S_btlazy2 && cp.windowLog > 14) ? (1u << cp.hashLog) / 16   // tag bytes of the row finder
+                     : (cp.strategy >= S_greedy) ? ((cp.strategy < S_btlazy2 && cp.windowLog > 14) ? (1u << cp.hashLog) / 16   // tag bytes of the row finder
                                                                         : (1u << cp.chainLog) / 4) : 0;  // chain table / binary tree
+        u32 const n3 = (cp.strategy >= S_btopt && cp.minMatch == 3) ? (1u << cp.windowLog) / 4 : 0;  // hash3 table (hashLog3 = windowLog <= 16)
         struct alignas(16) Q { u32 a, b, c, d; };
-        Q* const qL = reinterpret_cast<Q*>(W.hashLong); Q* const qS = reinterpret_cast<Q*>(W.hashSmall);
+        Q* const qL = reinterpret_cast<Q*>(W.hashLong); Q* const qS = reinterpret_cast<Q*>(W.hashSmall); Q* const q3 = reinterpret_cast<Q*>(W.hash3);
         Q const z = { 0, 0, 0, 0 };
         for (u32 i = (u32)w.lane; i < nL; i += C::W) qL[i] = z;
         for (u32 i = (u32)w.lane; i < nS; i += C::W) qS[i] = z;
+        for (u32 i = (u32)w.lane; i < n3; i += C::W) q3[i] = z;
         w.sync(); }
     u32 nbSeq = 0, lastLL = 0;
-    if (C::W > 1 && (ONLY == S_dfast || (ONLY == 0 && cp.strategy == S_dfast))) {
+    if (withOpt && (ONLY == ONLY_OPT || cp.strategy >= S_btopt)) {
+        if (w.lane == 0) nbSeq = parse_opt(W, src, srcSize, cp, &lastLL);
+        w.sync();
+        nbSeq = w.bcast(nbSeq); lastLL = w.bcast(lastLL);
+    } else if (C::W > 1 && (ONLY == S_dfast || (ONLY == 0 && cp.strategy == S_dfast))) {
         if (ONLY == S_dfast && cp.minMatch == 5) nbSeq = parse_dfast_warp<C, 5>(w, W, src, srcSize, cp.hashLog, cp.chainLog, 5, &lastLL);
         else nbSeq = parse_dfast_warp(w, W, src, srcSize, cp.hashLog, cp.chainLog, cp.minMatch, &lastLL);
     } else if (C::W > 1 && (ONLY == S_fast || (ONLY == 0 && cp.strategy == S_fast))) {
@@ -2305,7 +2769,7 @@ ZB_HDN size_t encode_stage(const C& w, EncShared& S, const EncWork& W, u8* dst, 
         // ZSTD_entropyCompressSeqStore_wExtLitBuffer :3005-3042
         if (cSize == ERR(E_dstSize_tooSmall) && srcSize <= cap - 3) cSize = 0;
         if (isErr(cSize)) return cSize;
-        if (cSize) { size_t const maxCSize = srcSize - ((srcSize >> 6) + 2); if (cSize >= maxCSize) cSize = 0; }
+        if (cSize) { size_t const maxCSize = srcSize - min_gain(srcSize, cp.strategy); if (cSize >= maxCSize) cSize = 0; }
     }
     if (cSize == 0) {   // ZSTD_noCompressBlock
         if (srcSize + 3 > cap) return ERR(E_dstSize_tooSmall);
