@@ -171,15 +171,19 @@ ZSTDB200_API zstdb200_ctx* zstdb200_create(int device);
 ZSTDB200_API void zstdb200_free(zstdb200_ctx* ctx);
 ZSTDB200_API const char* zstdb200_last_error(void);          /* thread-local text of the last CUDA/runtime failure */
 ZSTDB200_API int zstdb200_device_count(void);
-/* tuning knobs (also read from the environment at context creation):
- *   "enc_warps_per_sm" / ZSTDB200_ENC_WARPS_PER_SM, "dec_warps_per_sm" / ZSTDB200_DEC_WARPS_PER_SM,
- *   "parse_lanes" (4|8|16|32), "parse_blocks_per_sm", "lazy_blocks_per_sm" (4|6|8: residency of the levels >= 5 parse kernel),
- *   "parse_est_bytes" (prefix parsed for the cost estimate that orders the parse), "dec_pipeline" (0|1),
- *   "host_slices" / "host_slices_dec" (slices of the synchronous host-memory calls; defaults 1 / 2), "timing" (0|1),
- *   "entropy_overlap" (0|1, default 1 / ZSTDB200_ENTROPY_OVERLAP: the entropy stage is launched as a programmatic dependent of the parse and
+/* tuning knobs; returns 0, or -1 for an unknown name or a value out of the option's range:
+ *   "enc_warps_per_sm", "dec_warps_per_sm" (any value; <= 0: as many as shared memory allows),
+ *   "parse_lanes" (4|8|16|32), "parse_blocks_per_sm" (1..16), "lazy_blocks_per_sm" / "opt_blocks_per_sm" (4|6|8: residency of the
+ *   levels >= 5 / optimal-parser parse kernels), "parse_est_bytes" (256..65536: prefix parsed for the cost estimate that orders the parse),
+ *   "dec_pipeline" (0|1), "l2_fetch_granularity" (32|64|128),
+ *   "host_slices" / "host_slices_dec" (1..64: slices of the synchronous host-memory calls; defaults 1 / 2), "timing" (0|1),
+ *   "entropy_overlap" (0|1, default 1: the entropy stage is launched as a programmatic dependent of the parse and
  *   takes frames in the order their parse finishes, filling the SMs the parse's tail leaves idle),
- *   "kernel_fifo" (0|1, default 1 / ZSTDB200_KERNEL_FIFO: the kernel sections of host-memory operations queued on different work sets run
- *   one after the other in submission order -- copies still overlap them; two batches in the kernels at once only slow each other down) */
+ *   "kernel_fifo" (0|1, default 1: the kernel sections of host-memory operations queued on different work sets run
+ *   one after the other in submission order -- copies still overlap them; two batches in the kernels at once only slow each other down).
+ * zstdb200_create reads these ten from the environment (a value the option rejects is ignored): ZSTDB200_ENC_WARPS_PER_SM,
+ * ZSTDB200_DEC_WARPS_PER_SM, ZSTDB200_PARSE_LANES, ZSTDB200_PARSE_BLOCKS_PER_SM, ZSTDB200_LAZY_BLOCKS_PER_SM, ZSTDB200_PARSE_EST_BYTES,
+ * ZSTDB200_L2_FETCH (l2_fetch_granularity), ZSTDB200_HOST_SLICES, ZSTDB200_ENTROPY_OVERLAP and ZSTDB200_KERNEL_FIFO. */
 ZSTDB200_API int zstdb200_set_option(zstdb200_ctx* ctx, const char* name, long long value);
 ZSTDB200_API unsigned long long zstdb200_kernel_launches(const zstdb200_ctx* ctx);   /* kernels launched so far */
 /* with option "timing" = 1 every kernel launch is bracketed by CUDA events on its stream; this returns the averages
