@@ -186,6 +186,9 @@ ZSTDB200_API int zstdb200_device_count(void);
  * ZSTDB200_L2_FETCH (l2_fetch_granularity), ZSTDB200_HOST_SLICES, ZSTDB200_ENTROPY_OVERLAP and ZSTDB200_KERNEL_FIFO. */
 ZSTDB200_API int zstdb200_set_option(zstdb200_ctx* ctx, const char* name, long long value);
 ZSTDB200_API unsigned long long zstdb200_kernel_launches(const zstdb200_ctx* ctx);   /* kernels launched so far */
+/* frames of many blocks that zstdb200_decompress_batch gave to the segment decoder: regenerated there (deferred = 0), or handed to
+ * the fused kernel because the segment decoder could not vouch for them (deferred = 1: corrupted, short of capacity, wrong checksum) */
+ZSTDB200_API unsigned long long zstdb200_segment_frames(const zstdb200_ctx* ctx, int deferred);
 /* with option "timing" = 1 every kernel launch is bracketed by CUDA events on its stream; this returns the averages
  * since the previous call as "name:ms:count;..." (synchronises).  Used by bench.py for the roofline line. */
 ZSTDB200_API size_t zstdb200_kernel_times(zstdb200_ctx* ctx, char* buf, size_t cap);

@@ -107,6 +107,7 @@ def lib() -> C.CDLL:
     sig("zstdb200_device_count", i)
     sig("zstdb200_set_option", i, vp, C.c_char_p, C.c_longlong)
     sig("zstdb200_kernel_launches", C.c_ulonglong, vp)
+    sig("zstdb200_segment_frames", C.c_ulonglong, vp, i)
     sig("zstdb200_kernel_times", sz, vp, C.c_char_p, sz)
     sig("zstdb200_compress_chunks", sz, vp, i, vp, sz, sz, vp, sz, c_size_p, c_size_p)
     sig("zstdb200_decompress_frames", sz, vp, vp, c_size_p, sz, vp, sz, c_size_p)

@@ -237,6 +237,23 @@ struct SeqChain {
     ZB_HD bool plain() const { return k + 1 < nbSeq && (top >> 5) >= 8; }      // walk<true>() may take the next sequence
     ZB_HD bool clean(u32 floorBit) const { return top + 1 == (int)floorBit; }       // every bit consumed, none borrowed
 };
+// The value side of one raw record: both lengths, the offset selector (idx 0..2 = repcode slot, 3 = rep0 - 1, 4 = a new offset) and
+// the new offset the record would carry for idx 4.
+struct SeqVal { u32 litLength, matchLength, idx, ofNew; };
+ZB_HD SeqVal seq_value(SeqRaw const& r, const CodeTables* ct) {
+    u32 const llBits = r.a & 0xFF, ofBits = (r.a >> 8) & 0xFF, mlBits = r.b & 0xFF;
+    u32 const E = llBits + mlBits;
+    u32 const ofVal = shr_clamp(r.v0, 32 - ofBits);
+    u32 const x = shr_clamp(fshl32(r.v1, r.v0, ofBits & 31), 32 - E);
+    u32 const llc = (r.a >> 25) & 0x3F, mlc = (r.b >> 25) & 0x3F;
+    SeqVal s;
+    s.litLength = ct->LL_base[llc < MaxLL ? llc : MaxLL] + (x & ((1u << (llBits & 31)) - 1));
+    s.matchLength = ct->ML_base[mlc < MaxML ? mlc : MaxML] + (x >> (llBits & 31));
+    u32 const ll0 = (llc == 0);          // :1300 tests litLength base == 0, true for code 0 only
+    s.idx = ofBits > 1 ? 4u : ofBits + ll0 + ofVal;
+    s.ofNew = ((1u << (ofBits & 31)) - 3) + ofVal;
+    return s;
+}
 struct SeqValue {
     u32 rep0, rep1, rep2, k;
     u64* out;
@@ -245,17 +262,10 @@ struct SeqValue {
     // `ok` false: the record was not there yet -- everything is computed, nothing is kept (selects instead of a branch: the value
     // warp polls 14 rings at once and must not diverge on which of them had news)
     ZB_HD void take_if(bool ok, SeqRaw const& r, const CodeTables* ct) {
-        u32 const llBits = r.a & 0xFF, ofBits = (r.a >> 8) & 0xFF, mlBits = r.b & 0xFF;
-        u32 const E = llBits + mlBits;
-        u32 const ofVal = shr_clamp(r.v0, 32 - ofBits);
-        u32 const x = shr_clamp(fshl32(r.v1, r.v0, ofBits & 31), 32 - E);
-        u32 const llc = (r.a >> 25) & 0x3F, mlc = (r.b >> 25) & 0x3F;
-        u32 const litLength = ct->LL_base[llc < MaxLL ? llc : MaxLL] + (x & ((1u << (llBits & 31)) - 1));
-        u32 const matchLength = ct->ML_base[mlc < MaxML ? mlc : MaxML] + (x >> (llBits & 31));
+        SeqVal const s = seq_value(r, ct);
+        u32 const litLength = s.litLength, matchLength = s.matchLength, idx = s.idx;
         // offset / repcode history, all cases as selects: idx 0..3 = repcode slots (3: rep0 - 1), 4 = a new offset
-        u32 const ll0 = (llc == 0);          // :1300 tests litLength base == 0, true for code 0 only
-        u32 const idx = ofBits > 1 ? 4u : ofBits + ll0 + ofVal;
-        u32 cand = ((1u << (ofBits & 31)) - 3) + ofVal;   // selects, not branches: lanes of a warp take all five cases at once
+        u32 cand = s.ofNew;                  // selects, not branches: lanes of a warp take all five cases at once
         cand = idx == 0 ? rep0 : cand; cand = idx == 1 ? rep1 : cand; cand = idx == 2 ? rep2 : cand; cand = idx == 3 ? rep0 - 1 : cand;
         cand -= !cand;                       // only a repcode can be zero here (rep0 - 1, or a corrupted history)
         u32 const n2 = idx >= 2 ? rep1 : rep2, n1 = idx >= 1 ? rep0 : rep1;

@@ -1,0 +1,348 @@
+// zb_decode_segment.cuh -- decoder for one frame of many blocks, a segment (a run of whole blocks) at a time, every stage parallel
+// over the blocks of the segment or over its output bytes (kernels k_seg_* in zb_capi.cu):
+//
+//   A  seg_prepare  warp / block     literal and sequence section headers, the tables the block describes -> HBM, stream geometry
+//   B  seg_tables   one thread       in block order: the earlier block (or the carried state) whose table a repeating block reuses
+//   C  dec_huf      thread / stream  Huffman streams -> the block's literal buffer (zb_decode_fast.cuh)
+//      seg_seq      thread / block   sequence stream -> lengths and raw offset selectors, and the block's repcode summary
+//      seg_scan     one thread       output position of every block; the repcode history at every block start (summaries applied
+//                                    in block order)
+//      seg_offsets  thread / block   concrete offsets from the block's start history
+//   D  seg_fill     warp / block     link map: every output byte of the segment is a final byte or the segment byte it copies
+//      seg_jump     thread / byte    pointer jumping on the link map, in place, until every byte is final; the bytes -> dst
+//
+// Between segments the frame carries its output position, the repcode history and its last Huffman / FSE tables (SegCarry).  The
+// whole frame's output lies in dst, so copies reach back to the frame start, as in the fused decoder.
+//
+// The segment path decides no error itself.  Whatever the fused decoder could reject -- a stage status, a table repeated before any
+// block described it, a block regenerating more than blockSizeMax, an offset reaching before the frame, output beyond the capacity or
+// the content size, a wrong checksum -- marks the frame `bad`, and the caller decodes it again on the fused kernel, whose bytes or
+// error code are the result.  So valid frames decode to the same bytes and corrupted ones to the same error codes as before.
+#pragma once
+#include "zb_decode_fast.cuh"
+
+namespace zb {
+
+constexpr u32 SEG_HUF_ENTRIES = 1u << HUF_TABLELOG_MAX;
+constexpr u32 SEG_CARRY = 0xFFFFFFFFu;       // table source: the state carried in from the frame's earlier segments
+constexpr u32 SEG_NONE = 0xFFFFFFFEu;        // no table to reuse yet
+constexpr u32 SEG_FINAL = 0x80000000u;       // link map entry: final byte in the low 8 bits; otherwise the index of the segment byte copied
+constexpr u32 REP_LIT = 0xFFFFFFFFu;
+
+// A repcode slot as a function of the history {in[0], in[1], in[2]} at the block's start: k == REP_LIT: the literal offset v; otherwise
+// in[v] after k times `rep0 - 1` (ZSTD_decodeSequence :1300-1310: the result 0 becomes -1, `temp -= !temp`).  History values are never 0.
+struct RepSym { u32 v, k; };
+ZB_HD u32 rep_dec(u32 x, u32 k) { return x > k ? x - k : 0xFFFFFFFFu - (k - x); }
+ZB_HD u32 rep_eval(RepSym s, const u32* in) { return s.k == REP_LIT ? s.v : rep_dec(in[s.v], s.k); }
+// One sequence's offset selector: idx 0..2 = repcode slot, 3 = rep0 - 1, 4 = the new offset v.  Returns the offset taken.
+ZB_HD u32 rep_step(u32* r, u32 idx, u32 v) {
+    u32 const c = idx == 4 ? v : idx == 3 ? rep_dec(r[0], 1) : r[idx];
+    if (idx >= 2) r[2] = r[1];
+    if (idx >= 1) r[1] = r[0];
+    r[0] = c;
+    return c;
+}
+ZB_HD void rep_step_sym(RepSym* r, u32 idx, u32 v) {
+    RepSym c = r[idx < 3 ? idx : 0];
+    if (idx == 4) { c.v = v; c.k = REP_LIT; }
+    else if (idx == 3) { if (c.k == REP_LIT) c.v = rep_dec(c.v, 1); else c.k += 1; }
+    if (idx >= 2) r[2] = r[1];
+    if (idx >= 1) r[1] = r[0];
+    r[0] = c;
+}
+
+struct SegBlock {
+    DecDesc d;           // as in the staged decoder; blockOff relative to the frame, mode 1 compressed / 2 raw / 3 rle
+    u32 litType;         // literals block type of a compressed block (3: the previous Huffman table again)
+    u32 seqModes;        // symbol compression modes byte (a field of 3: the previous table again), 0 without sequences
+    u32 hufSrc, fseSrc[3];    // segment block whose table the block uses, or SEG_CARRY
+    u32 bad;             // the frame goes to the fused decoder
+    u32 regen;
+    u64 out;             // frame position of the block's first output byte
+    u64 sumLL, sumML;
+    u32 rep[3];          // repcode history at the block's start
+    RepSym sum[3];       // ... and at its end, as functions of rep
+};
+
+struct SegCarry {
+    u64 pos, cap;        // output bytes of the frame so far, output capacity of the item
+    u32 bad;
+    u32 hasHuf, hufLog, hasFse, fseLog[3];
+    u32 rep[3];
+    u32 nextHuf, nextFse[3];  // the last describing blocks of the segment just prepared (SEG_CARRY / SEG_NONE: none there)
+    u16 huf[SEG_HUF_ENTRIES];
+    u32 fse[FAST_FSE_ENTRIES];
+};
+
+// The largest window the segment decoder takes (the default windowLogMax): larger ones stay with the fused decoder.
+constexpr u64 SEG_WINDOW_MAX = 1ull << 27;
+
+// Host side: the blocks of an item that is exactly one frame of more than one block -- magic number, no dictionary, a window of at most
+// SEG_WINDOW_MAX, every block inside the item, the checksum (when the frame has one) its last four bytes.  Returns the number of blocks
+// (0: the item is not such a frame); refs[k] = offset of block k's header | that header << 32, *xxh = the stored checksum.
+ZB_HDN u32 seg_walk(const u8* src, size_t size, FrameHeader* fh, u64* refs, u32* xxh) {
+    if (size < 9 || size > 0xFFFFFFFFu || load32(src) != MAGIC) return 0;
+    if (read_frame_header(fh, src, size) != 0 || fh->skippable || fh->dictID || fh->windowSize > SEG_WINDOW_MAX) return 0;
+    size_t pos = fh->headerSize; u32 n = 0;
+    for (;;) {
+        if (size - pos < 3) return 0;
+        u32 const bh = load24(src + pos), type = (bh >> 1) & 3;
+        size_t const cSize = type == 1 ? 1 : bh >> 3;
+        if (type == 3 || cSize > size - pos - 3) return 0;
+        if (refs) refs[n] = (u64)pos | ((u64)bh << 32);
+        n++; pos += 3 + cSize;
+        if (bh & 1) break;
+    }
+    if (size - pos != (fh->checksum ? 4u : 0u) || n < 2) return 0;
+    *xxh = fh->checksum ? load32(src + pos) : 0;
+    return n;
+}
+
+// ---------------------------------------------------------------------------------------- stage A
+// `bh` = the block header; the block's content starts at frame + off + 3.
+template <class C>
+ZB_HDN void seg_prepare(const C& w, DecShared& S, const u8* frame, u32 off, u32 bh, u32 blockSizeMax, SegBlock* b, u16* hufOut, u32* fseOut) {
+    SegBlock B;
+    memset(&B, 0, sizeof B);
+    DecDesc& L = B.d;
+    L.outMax = 0xFFFFFFFFu;
+    u32 const type = (bh >> 1) & 3, cSize = bh >> 3;
+    L.blockOff = off + 3; L.cSize = type == 1 ? 1 : cSize;
+    do {
+        if (type == 0) { L.mode = 2; L.regen = cSize; break; }
+        if (type == 1) { L.mode = 3; L.regen = cSize; L.rleByte = frame[off + 3]; break; }
+        L.mode = 1;
+        if (type == 3 || cSize > blockSizeMax || cSize < 2) { B.bad = 1; break; }
+        const u8* const blk = frame + off + 3;
+        if (w.lane == 0) { S.litEntropy = 1; S.fseEntropy = 1; }      // repeats are resolved by seg_tables
+        w.sync();
+        B.litType = blk[0] & 3;
+        LitInfo li;
+        memset(&li, 0, sizeof li);
+        size_t const lr = parse_literals(w, S, blk, cSize, blockSizeMax, blockSizeMax, &li);
+        if (isErr(lr)) { B.bad = 1; break; }
+        L.litMode = li.mode; L.litSize = li.litSize; L.rawOff = li.rawOff; L.rleByte = li.rleByte; L.nStreams = li.nStreams;
+        for (int k = 0; k < 4; k++) { L.sOff[k] = li.sOff[k]; L.sLen[k] = li.sLen[k]; L.oOff[k] = li.oOff[k]; L.oCnt[k] = li.oCnt[k]; }
+        if (li.mode == 2) {
+            if (B.litType == 2) {
+                L.hufLog = S.hufLog;
+                for (u32 i = (u32)w.lane; i < (1u << S.hufLog); i += C::W) hufOut[i] = S.huf[i];
+            }
+            for (u32 k = 0; k < li.nStreams; k++) {
+                u32 const last = li.sLen[k] ? blk[li.sOff[k] + li.sLen[k] - 1] : 0;
+                if (last == 0) { B.bad = 1; break; }
+                L.sBits[k] = (li.sLen[k] - 1) * 8 + highbit32(last);
+            }
+            if (B.bad) break;
+        }
+        int nbSeq = 0;
+        size_t const hr = parse_seq_section(w, S, blk + lr, cSize - lr, 1, &nbSeq);
+        if (isErr(hr) || (u32)nbSeq > FAST_MAXS) { B.bad = 1; break; }
+        L.nbSeq = (u32)nbSeq; L.seqOff = (u32)(lr + hr); L.seqLen = (u32)(cSize - lr - hr);
+        if (nbSeq) {
+            u32 const b0 = blk[lr];
+            B.seqModes = blk[lr + (b0 < 0x80 ? 1 : b0 == 0xFF ? 3 : 2)];
+            u32* const logs[3] = { &L.logLL, &L.logOF, &L.logML };
+            for (int t = 0; t < 3; t++) {
+                if (((B.seqModes >> (6 - 2 * t)) & 3) == 3) continue;
+                *logs[t] = S.fseLog[t];
+                u32* const out = fseOut + (t == 0 ? 0 : t == 1 ? FAST_FSE_OF : FAST_FSE_ML);
+                for (u32 i = (u32)w.lane; i < (1u << S.fseLog[t]); i += C::W) {
+                    u32 const e = S.fse[t][i], sym = e >> 24;
+                    out[i] = fse2_pack(e, t == 0 ? ZB_T.LL_bits[sym] : t == 1 ? sym : ZB_T.ML_bits[sym]);
+                }
+            }
+            u32 const last = L.seqLen ? blk[L.seqOff + L.seqLen - 1] : 0;
+            if (last == 0) { B.bad = 1; break; }
+            L.seqBits = (L.seqLen - 1) * 8 + highbit32(last);
+        }
+    } while (0);
+    w.sync();
+    if (w.lane == 0) *b = B;
+    w.sync();
+}
+
+// ---------------------------------------------------------------------------------------- stage B
+// In block order: the table every repeating block reuses (ZSTD_decodeLiteralsBlock :148 / ZSTD_buildSeqTable :686).  The first
+// segment of a frame starts the carried state.
+ZB_HDN void seg_tables(SegBlock* blocks, u32 n, SegCarry* c, bool first, u64 cap) {
+    if (first) {
+        c->pos = 0; c->cap = cap; c->bad = 0; c->hasHuf = 0; c->hasFse = 0;
+        c->rep[0] = 1; c->rep[1] = 4; c->rep[2] = 8;
+    }
+    u32 huf = c->hasHuf ? SEG_CARRY : SEG_NONE, fse[3];
+    for (int t = 0; t < 3; t++) fse[t] = c->hasFse ? SEG_CARRY : SEG_NONE;
+    for (u32 j = 0; j < n && !c->bad; j++) {
+        SegBlock& B = blocks[j];
+        if (B.bad) { c->bad = 1; break; }
+        if (B.d.mode != 1) continue;
+        if (B.litType == 3) {
+            if (huf == SEG_NONE) { c->bad = 1; break; }
+            B.hufSrc = huf; B.d.hufLog = huf == SEG_CARRY ? c->hufLog : blocks[huf].d.hufLog;
+        } else if (B.litType == 2) huf = j;
+        if (B.d.nbSeq) {
+            u32* const logs[3] = { &B.d.logLL, &B.d.logOF, &B.d.logML };
+            for (int t = 0; t < 3; t++) {
+                if (((B.seqModes >> (6 - 2 * t)) & 3) == 3) {
+                    if (fse[t] == SEG_NONE) { c->bad = 1; break; }
+                    *logs[t] = fse[t] == SEG_CARRY ? c->fseLog[t] : (t == 0 ? blocks[fse[t]].d.logLL : t == 1 ? blocks[fse[t]].d.logOF : blocks[fse[t]].d.logML);
+                } else fse[t] = j;
+                B.fseSrc[t] = fse[t];
+            }
+        }
+    }
+    c->nextHuf = huf;
+    for (int t = 0; t < 3; t++) c->nextFse[t] = fse[t];
+}
+
+// ---------------------------------------------------------------------------------------- stage C
+// Huffman stream k of block j, with the table the block uses.
+ZB_HDN void seg_huf(SegBlock* blocks, u32 j, int k, const u8* frame, const u16* hufBase, const SegCarry* c, u8* lit) {
+    SegBlock& B = blocks[j];
+    u32 const src = B.litType == 3 ? B.hufSrc : j;
+    dec_huf(&B.d, k, frame + B.d.blockOff, src == SEG_CARRY ? c->huf : hufBase + (size_t)src * SEG_HUF_ENTRIES, lit);
+}
+
+// Block j's sequence stream: lengths | selector << 36 to seqs, the new offset of a selector 4 to offs; the summary of its repcodes.
+ZB_HDN void seg_seq(SegBlock* blocks, u32 j, const u8* frame, const u32* fseBase, const SegCarry* c, u64* seqs, u32* offs) {
+    SegBlock& B = blocks[j];
+    for (u32 s = 0; s < 3; s++) { B.sum[s].v = s; B.sum[s].k = 0; }
+    B.sumLL = 0; B.sumML = 0;
+    if (B.d.mode != 1 || B.d.nbSeq == 0) return;
+    const u32* t[3];
+    u32 const tOff[3] = { 0, FAST_FSE_OF, FAST_FSE_ML };
+    for (int k = 0; k < 3; k++) t[k] = (B.fseSrc[k] == SEG_CARRY ? c->fse : fseBase + (size_t)B.fseSrc[k] * FAST_FSE_ENTRIES) + tOff[k];
+    MemWords ws; ws.g.set(frame + B.d.blockOff + B.d.seqOff);
+    SeqChain D;
+    D.begin(ws, ws.g.floorBit, B.d.seqBits, B.d.logLL, B.d.logOF, B.d.logML, B.d.nbSeq);
+    RepSym sum[3] = { { 0, 0 }, { 1, 0 }, { 2, 0 } };
+    u64 sLL = 0, sML = 0;
+    const CodeTables* const ct = &ZB_T;
+    for (u32 k = 0; D.more(); k++) {
+        SeqRaw const r = D.plain() ? D.walk<true>(ws, t[0], t[1], t[2]) : D.walk<false>(ws, t[0], t[1], t[2]);
+        SeqVal const s = seq_value(r, ct);          // the offset stays a selector until the block's start history is known
+        u64 const l = umin(s.litLength, 0x3FFFFu), m = umin(s.matchLength, 0x3FFFFu);
+        seqs[k] = l | (m << 18) | ((u64)s.idx << 36);
+        offs[k] = s.ofNew;
+        rep_step_sym(sum, s.idx, s.ofNew);
+        sLL += l; sML += m;
+    }
+    if (!D.clean(ws.g.floorBit)) B.bad = 1;
+    for (int s = 0; s < 3; s++) B.sum[s] = sum[s];
+    B.sumLL = sLL; B.sumML = sML;
+}
+
+// Output positions and start histories, in block order (after stage C); `last`: the frame's final segment.
+ZB_HDN void seg_scan(SegBlock* blocks, u32 n, SegCarry* c, u32 blockSizeMax) {
+    if (c->bad) return;
+    u64 pos = c->pos;
+    u32 rep[3] = { c->rep[0], c->rep[1], c->rep[2] };
+    for (u32 j = 0; j < n; j++) {
+        SegBlock& B = blocks[j];
+        u64 regen = B.d.regen;
+        if (B.d.mode == 1) {
+            if (B.bad || B.d.stB || B.d.stC || B.sumLL > B.d.litSize) { c->bad = 1; return; }
+            regen = B.d.litSize + B.sumML;
+        }
+        if (regen > blockSizeMax || regen > c->cap - pos) { c->bad = 1; return; }
+        B.regen = (u32)regen; B.out = pos; pos += regen;
+        for (int s = 0; s < 3; s++) B.rep[s] = rep[s];
+        if (B.d.mode == 1 && B.d.nbSeq) {
+            u32 nr[3];
+            for (int s = 0; s < 3; s++) nr[s] = rep_eval(B.sum[s], rep);
+            for (int s = 0; s < 3; s++) rep[s] = nr[s];
+        }
+    }
+    c->pos = pos;
+    for (int s = 0; s < 3; s++) c->rep[s] = rep[s];
+}
+
+// Block j: concrete offsets from its start history, in place over the new offsets.
+ZB_HDN void seg_offsets(const SegBlock* blocks, u32 j, const u64* seqs, u32* offs) {
+    SegBlock const& B = blocks[j];
+    if (B.d.mode != 1) return;
+    u32 r[3] = { B.rep[0], B.rep[1], B.rep[2] };
+    for (u32 k = 0; k < B.d.nbSeq; k++) offs[k] = rep_step(r, (u32)(seqs[k] >> 36), offs[k]);
+}
+
+// The tables the next segment may reuse, into the carried state (after stage C read the old ones).
+template <class C>
+ZB_HD void seg_carry_tables(const C& w, const SegBlock* blocks, const u16* hufBase, const u32* fseBase, SegCarry* c) {
+    if (c->bad) return;
+    if (c->nextHuf < SEG_NONE) {
+        u32 const j = c->nextHuf;
+        for (u32 i = (u32)w.lane; i < SEG_HUF_ENTRIES; i += C::W) c->huf[i] = hufBase[(size_t)j * SEG_HUF_ENTRIES + i];
+        if (w.lane == 0) { c->hufLog = blocks[j].d.hufLog; c->hasHuf = 1; }
+    }
+    u32 const tOff[3] = { 0, FAST_FSE_OF, FAST_FSE_ML }, tLen[3] = { 512, 256, 512 };
+    for (int t = 0; t < 3; t++) {
+        if (c->nextFse[t] >= SEG_NONE) continue;
+        u32 const j = c->nextFse[t];
+        for (u32 i = (u32)w.lane; i < tLen[t]; i += C::W) c->fse[tOff[t] + i] = fseBase[(size_t)j * FAST_FSE_ENTRIES + tOff[t] + i];
+        if (w.lane == 0) { c->fseLog[t] = t == 0 ? blocks[j].d.logLL : t == 1 ? blocks[j].d.logOF : blocks[j].d.logML; c->hasFse = 1; }
+    }
+    w.sync();
+}
+
+// ---------------------------------------------------------------------------------------- stage D
+// Block j's bytes into the link map of the segment that starts at frame position segStart: literal bytes and bytes copied from before
+// the segment are final, a match byte inside the segment names the byte it copies -- for a match that overlaps itself, the byte of its
+// first period, so that a run is one link deep.  Sequences go 32 at a time, their bytes are spread over the lanes.
+struct SegRec { u64 o, md; u32 ls, off; };
+template <class C>
+ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const u8* frame, const u8* lit, const u64* seqs, const u32* offs,
+                     const u8* dst, u64 segStart, u32* link, SegCarry* c) {
+    SegBlock const& B = blocks[j];
+    u64 const base = B.out;
+    auto put = [&](u64 p, u32 v) { link[p - segStart] = v; };
+    if (B.d.mode == 2 || B.d.mode == 3) {
+        const u8* const s = frame + B.d.blockOff;
+        for (u32 i = (u32)w.lane; i < B.regen; i += C::W) put(base + i, SEG_FINAL | (B.d.mode == 2 ? s[i] : B.d.rleByte));
+        w.sync();
+        return;
+    }
+    const u8* const L = B.d.litMode == 0 ? frame + B.d.blockOff + B.d.rawOff : lit;
+    bool const rle = B.d.litMode == 1;
+    u64 op = base; u32 lp = 0;
+    for (u32 s0 = 0; s0 < B.d.nbSeq; s0 += C::W) {
+        u32 const i = s0 + (u32)w.lane;
+        u64 const q = i < B.d.nbSeq ? seqs[i] : 0;
+        u32 const ll = (u32)(q & 0x3FFFF), ml = (u32)((q >> 18) & 0x3FFFF), off = i < B.d.nbSeq ? offs[i] : 0;
+        u64 const o = op + w.exscan(ll + ml);
+        u32 const ls = lp + w.exscan(ll);
+        bool const bad = i < B.d.nbSeq && (u64)off > o + ll;        // the copy would start before the frame (ZSTD_execSequence :1034)
+        if (w.ballot(bad)) { if (w.lane == 0) c->bad = 1; return; }
+        SegRec r; r.o = o; r.md = o + ll; r.ls = ls; r.off = off;
+        R[w.lane] = r;
+        u32 const cnt = B.d.nbSeq - s0 < (u32)C::W ? B.d.nbSeq - s0 : (u32)C::W;
+        u64 const end = w.shfl(o + ll + ml, (int)cnt - 1);
+        u32 const lend = w.shfl(ls + ll, (int)cnt - 1);
+        w.sync();
+        u32 u = 0;
+        for (u64 p = op + (u32)w.lane; p < end; p += C::W) {
+            while (u + 1 < cnt && R[u + 1].o <= p) u++;       // bytes of a lane only move forward
+            SegRec const& e = R[u];
+            u32 v;
+            if (p < e.md) v = SEG_FINAL | (rle ? B.d.rleByte : L[e.ls + (u32)(p - e.o)]);
+            else {
+                u64 const src = e.md - e.off + (p - e.md) % e.off;
+                v = src < segStart ? SEG_FINAL | dst[src] : (u32)(src - segStart);
+            }
+            put(p, v);
+        }
+        w.sync();
+        op = end; lp = lend;
+    }
+    for (u32 k = (u32)w.lane; k < B.d.litSize - lp; k += C::W) put(op + k, SEG_FINAL | (rle ? B.d.rleByte : L[lp + k]));
+    w.sync();
+}
+
+// Segment byte p: follows its links, shortening its own entry on the way (others that reach it later jump further), until a final
+// byte.  Every link points to an earlier byte, so the walk ends; an entry only ever changes to another entry on its own chain.
+ZB_HD u8 seg_jump(volatile u32* link, u32 p) {
+    u32 v = link[p];
+    while (!(v & SEG_FINAL)) { v = link[v]; link[p] = v; }
+    return (u8)v;
+}
+
+}  // namespace zb
