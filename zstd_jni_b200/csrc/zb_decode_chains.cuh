@@ -311,13 +311,13 @@ __device__ __forceinline__ void chains_huf_warp(const ChainsArgs& a, unsigned ch
                         mbar_expect_tx(bar, bytes);
                         bulk_g2s(tabAddr, a.hufBase + (size_t)item * FAST_HUF_ENTRIES, bytes, bar);
                     }
-                    u32 const bits = k < (int)d->nStreams ? d->sBits[k] : HUF_UNUSABLE;
+                    u32 const bits = k < (int)d->nStreams ? d->sBits[k] : NO_END_MARK;
                     const u8* const blk = a.srcBase + a.srcOff[item] + d->blockOff;
-                    if (bits != HUF_UNUSABLE) ws.start(blk + d->sOff[k], bits);
+                    if (bits != NO_END_MARK) ws.start(blk + d->sOff[k], bits);
                     bool const landed = __all_sync(gmask, mbar_wait(bar, parity));      // (one verdict per group)
                     parity ^= 1;
                     if (!landed) { d->stB = E_GENERIC; exhausted = true; }
-                    else if (bits != HUF_UNUSABLE) {
+                    else if (bits != NO_END_MARK) {
                         H.begin(ws, ws.g.floorBit, bits, a.litBase + (size_t)item * a.litStride + d->oOff[k], d->oCnt[k]);
                         sh = 32 - log;
                         live = H.left != 0;

@@ -4,8 +4,8 @@
 // states of the sequence stream) are the critical path.  This pipeline gives every chain its own *thread*, runs
 // all of them at once next to each other, and then executes the sequences with whole warps:
 //
-//   A  dec_prepare   warp / frame    frame + block + section headers, Huffman and FSE decode tables -> HBM,
-//                                    bit lengths of every backward stream
+//   A  dec_prepare   warp / frame    frame_walk: one frame of one block; prepare_block (shared with the segment decoder): section
+//                                    headers, Huffman and FSE decode tables -> HBM, bit lengths of every backward stream
 //   B  HufChain      thread / stream 4 x n chains, each decodes one Huffman stream into the literal buffer   } one persistent
 //   C  SeqChain      thread / frame  sequence bitstream -> (litLength, matchLength, offset) packed in 8 B   } kernel (k_dec_chains)
 //   D  dec_exec      warp / frame    "byte gather": every output byte finds its sequence and its source byte,
@@ -33,7 +33,16 @@ constexpr u32 FAST_HUF_LOG = 11;            // largest Huffman table the staged 
 constexpr u32 FAST_HUF_ENTRIES = 1u << FAST_HUF_LOG;
 constexpr u32 FAST_FSE_ENTRIES = 512 + 256 + 512;  // LL | OF | ML
 constexpr u32 FAST_FSE_OF = 512, FAST_FSE_ML = 768;
-constexpr u32 HUF_UNUSABLE = 0xFFFFFFFFu;
+// FSE table t (0 LL, 1 OF, 2 ML) of a frame's or a block's FAST_FSE_ENTRIES cells: cells [fse_at(t), fse_at(t + 1))
+ZB_HD u32 fse_at(int t) { constexpr u32 at[4] = { 0, FAST_FSE_OF, FAST_FSE_ML, FAST_FSE_ENTRIES }; return at[t]; }
+constexpr u32 NO_END_MARK = 0xFFFFFFFFu;
+
+// Bits of the backward stream p[0, len) below its end mark, the highest set bit of its last byte.  NO_END_MARK: the stream is empty or
+// its last byte is zero, which BIT_initDStream (HUF_decompress1X1, ZSTD_decompressSequences) rejects as corruption.
+ZB_HD u32 end_mark_bits(const u8* p, u32 len) {
+    u32 const last = len ? p[len - 1] : 0u;
+    return last ? (len - 1) * 8 + highbit32(last) : NO_END_MARK;
+}
 
 // FSE cell of the staged path: extra bits of the code (bits 0..7) | nbBits (8..15) | new-state base (16..24) | code (25..30).
 // The byte-aligned bit counts make the sum of the three cells of a sequence carry both totals at once
@@ -47,93 +56,115 @@ struct DecDesc {
     u32 contentSize;
     u32 litMode, litSize, rawOff, rleByte, hufLog, nStreams;
     u32 sOff[4], sLen[4], oOff[4], oCnt[4];      // relative to the block content / the literal buffer
-    u32 sBits[4];                                // bits of Huffman stream k below its end mark (HUF_UNUSABLE: no end mark)
+    u32 sBits[4];                                // bits of Huffman stream k below its end mark (NO_END_MARK: none)
     u32 nbSeq, seqOff, seqLen;                   // sequence bitstream inside the block content
     u32 seqBits;                                 // bits of the sequence stream below its end mark
-    u32 logLL, logOF, logML;
+    union {                                      // the three FSE table logs, by table index or by name
+        u32 fseLog[3];
+        struct { u32 logLL, logOF, logML; };
+    };
     u32 regen;
     u32 hufLitSize;      // litSize when the literals are Huffman coded, else 0 (sort key of the Huffman chains)
     u32 seqUnusable;     // the sequence stream has no end mark: stC is final, nothing is decoded or executed
     u32 outMax;          // most bytes the compressed block may write (block_output_limit), 0xFFFFFFFF: the capacity
 };
+// k_dec_chains and k_order read these fields (k_order through a stride of sizeof(DecDesc) / 4): keeping the layout keeps their code
+static_assert(sizeof(DecDesc) == 184 && offsetof(DecDesc, sBits) == 124 && offsetof(DecDesc, nbSeq) == 140 && offsetof(DecDesc, seqBits) == 152 &&
+              offsetof(DecDesc, fseLog) == 156 && offsetof(DecDesc, hufLitSize) == 172 && offsetof(DecDesc, seqUnusable) == 176, "DecDesc layout");
 
 // ---------------------------------------------------------------------------------------- stage A
+// The blocks of an item that is exactly one frame of at most maxBlocks blocks: magic number, no dictionary, every block inside the item,
+// the checksum (when the frame has one) its last four bytes.  Returns the number of blocks (0: the item is not such a frame);
+// refs[k] = offset of block k's header | that header << 32 (refs may be null), *xxh = the stored checksum.
+ZB_HDN u32 frame_walk(const u8* src, size_t size, FrameHeader* fh, u32 maxBlocks, u64* refs, u32* xxh) {
+    if (size < 9 || size > 0xFFFFFFFFu || load32(src) != MAGIC) return 0;
+    if (read_frame_header(fh, src, size) != 0 || fh->skippable || fh->dictID) return 0;
+    size_t pos = fh->headerSize; u32 n = 0;
+    for (;;) {
+        if (size - pos < 3 || n == maxBlocks) return 0;
+        u32 const bh = load24(src + pos), type = (bh >> 1) & 3;
+        size_t const cSize = type == 1 ? 1 : bh >> 3;
+        if (type == 3 || cSize > size - pos - 3) return 0;
+        if (refs) refs[n] = (u64)pos | ((u64)bh << 32);
+        n++; pos += 3 + cSize;
+        if (bh & 1) break;
+    }
+    if (size - pos != (fh->checksum ? 4u : 0u)) return 0;
+    *xxh = fh->checksum ? load32(src + pos) : 0;
+    return n;
+}
+
+// One block of an item (both decoders): `bh` = its header, at item + off.  Describes it in L -- raw / rle, or for a compressed block the
+// literal geometry, the Huffman and sequence stream bits, the stage statuses, seqUnusable and outMax -- and copies out the tables the
+// block itself describes: the Huffman table when the literals carry one, every FSE table that is not a repeat.  Whether a repeat is
+// legal is the caller's S.litEntropy / S.fseEntropy.  Returns false, the block not described, when its Huffman table is larger than
+// 2^hufLogMax (the caller's table stride) or it has more than FAST_MAXS sequences.
+template <class C>
+ZB_HD bool prepare_block(const C& w, DecShared& S, const u8* item, u32 off, u32 bh, u32 blockSizeMax, size_t dstCapacity, u32 hufLogMax,
+                         DecDesc& L, u16* hufOut, u32* fseOut) {
+    u32 const type = (bh >> 1) & 3, cSize = type == 1 ? 1 : bh >> 3;
+    const u8* const blk = item + off + 3;
+    L.blockOff = off + 3; L.cSize = cSize;
+    if (type == 0) { L.mode = 2; L.regen = cSize; return true; }
+    if (type == 1) { L.mode = 3; L.regen = bh >> 3; L.rleByte = blk[0]; return true; }
+    // compressed block: from here on errors are recorded as the stage statuses
+    L.mode = 1;
+    if (cSize > blockSizeMax) { L.stA1 = E_srcSize_wrong; return true; }
+    LitInfo li{};
+    size_t const lr = parse_literals(w, S, blk, cSize, blockSizeMax, dstCapacity, &li);
+    if (isErr(lr)) { L.stA1 = (u32)(0 - lr); return true; }
+    bool const tree = (blk[0] & 3) == 2;
+    if (tree && S.hufLog > hufLogMax) return false;
+    if (dstCapacity > block_output_limit(dstCapacity, blockSizeMax, li.litSize, li.mode == 0 && lr + LIT_MARGIN <= cSize))
+        L.outMax = blockSizeMax + (u32)LIT_MARGIN;
+    L.litMode = li.mode; L.litSize = li.litSize; L.rawOff = li.rawOff; L.rleByte = li.rleByte; L.nStreams = li.nStreams;
+    for (int k = 0; k < 4; k++) { L.sOff[k] = li.sOff[k]; L.sLen[k] = li.sLen[k]; L.oOff[k] = li.oOff[k]; L.oCnt[k] = li.oCnt[k]; }
+    if (tree) {
+        L.hufLog = S.hufLog;
+        for (u32 i = (u32)w.lane; i < (1u << S.hufLog); i += C::W) hufOut[i] = S.huf[i];
+    }
+    if (li.mode == 2) {
+        L.hufLitSize = li.litSize;
+        for (u32 k = 0; k < li.nStreams; k++) {
+            L.sBits[k] = end_mark_bits(blk + li.sOff[k], li.sLen[k]);
+            if (L.sBits[k] == NO_END_MARK) L.stB = E_corruption_detected;
+        }
+    }
+    int nbSeq = 0;
+    size_t const hr = parse_seq_section(w, S, blk + lr, cSize - lr, dstCapacity, &nbSeq);
+    if (isErr(hr)) { L.stA2 = (u32)(0 - hr); return true; }
+    if ((u32)nbSeq > FAST_MAXS) return false;
+    L.nbSeq = (u32)nbSeq; L.seqOff = (u32)(lr + hr); L.seqLen = (u32)(cSize - lr - hr);
+    if (nbSeq == 0) return true;
+    for (int t = 0; t < 3; t++) {
+        if (S.fseMode[t] == 3) continue;
+        L.fseLog[t] = S.fseLog[t];
+        u32* const out = fseOut + fse_at(t);
+        for (u32 i = (u32)w.lane; i < (1u << S.fseLog[t]); i += C::W) {
+            u32 const e = S.fse[t][i], sym = e >> 24;
+            out[i] = fse2_pack(e, t == 0 ? ZB_T.LL_bits[sym] : t == 1 ? sym : ZB_T.ML_bits[sym]);
+        }
+    }
+    u32 const bits = end_mark_bits(blk + L.seqOff, L.seqLen);
+    if (bits == NO_END_MARK) { L.stC = E_corruption_detected; L.seqUnusable = 1; }
+    else L.seqBits = bits;
+    return true;
+}
+
+// The staged decoder takes an item that is one frame of one block, with its content size (at most one block) and no checksum.
 // All lanes of a warp; S is the warp's shared scratch; tables are copied out to hufOut / fseOut.
 template <class C>
 ZB_HDN void dec_prepare(const C& w, DecShared& S, const u8* src, size_t srcSize, size_t dstCapacity, DecDesc* d, u16* hufOut, u32* fseOut) {
-    DecDesc L;   // built in registers/local, stored by lane 0 at the end
-    L.mode = 0; L.stA1 = L.stB = L.stA2 = L.stC = L.stD = 0; L.regen = 0; L.nbSeq = 0; L.litMode = 0; L.litSize = 0; L.nStreams = 0;
-    L.blockOff = L.cSize = L.contentSize = L.rawOff = L.rleByte = L.hufLog = L.seqOff = L.seqLen = L.seqBits = L.logLL = L.logOF = L.logML = 0;
-    for (int k = 0; k < 4; k++) { L.sOff[k] = L.sLen[k] = L.oOff[k] = L.oCnt[k] = L.sBits[k] = 0; }
-    L.seqUnusable = 0; L.hufLitSize = 0; L.outMax = 0xFFFFFFFFu;
-    do {
-        if (srcSize < 9) break;
-        if (load32(src) != MAGIC) break;
-        FrameHeader fh;
-        size_t const r = read_frame_header(&fh, src, srcSize);
-        if (r != 0 || fh.skippable || fh.checksum || !fh.hasContentSize || fh.dictID != 0) break;
-        if (fh.contentSize > BLOCKSIZE_MAX) break;
-        if (srcSize < fh.headerSize + 3) break;
-        const u8* const bp = src + fh.headerSize;
-        u32 const bh = load24(bp), type = (bh >> 1) & 3; size_t cSize = bh >> 3;
-        if (!(bh & 1) || type == 3) break;
-        if (type == 1) cSize = 1;
-        if (fh.headerSize + 3 + cSize != srcSize) break;        // exactly one frame, one block
-        L.blockOff = fh.headerSize + 3; L.cSize = (u32)cSize; L.contentSize = (u32)fh.contentSize;
-        if (type == 0) { L.mode = 2; L.regen = (u32)cSize; break; }
-        if (type == 1) { L.mode = 3; L.regen = bh >> 3; L.rleByte = bp[3]; break; }
-        // compressed block: from here on the item is ours, errors are recorded instead of punting
-        L.mode = 1;
-        const u8* const blk = bp + 3;
-        if (cSize > fh.blockSizeMax) { L.stA1 = E_srcSize_wrong; break; }
-        if (w.lane == 0) { S.litEntropy = 0; S.fseEntropy = 0; }
+    DecDesc L{};         // built in registers/local, stored by lane 0 at the end; mode 0: the fused kernel decodes the item
+    L.outMax = 0xFFFFFFFFu;
+    FrameHeader fh; u64 ref; u32 xxh;
+    if (frame_walk(src, srcSize, &fh, 1, &ref, &xxh) && !fh.checksum && fh.hasContentSize && fh.contentSize <= BLOCKSIZE_MAX) {
+        L.contentSize = (u32)fh.contentSize;
+        if (w.lane == 0) { S.litEntropy = 0; S.fseEntropy = 0; }      // no earlier block: a repeated table is an error
         w.sync();
-        LitInfo li;
-        size_t const lr = parse_literals(w, S, blk, cSize, fh.blockSizeMax, dstCapacity, &li);
-        if (isErr(lr)) { L.stA1 = (u32)(0 - lr); break; }
-        if (li.mode == 2 && S.hufLog > FAST_HUF_LOG) { L.mode = 0; break; }     // legal, never written by the reference: fused kernel
-        if (dstCapacity > block_output_limit(dstCapacity, fh.blockSizeMax, li.litSize, li.mode == 0 && lr + LIT_MARGIN <= cSize))
-            L.outMax = fh.blockSizeMax + (u32)LIT_MARGIN;
-        L.litMode = li.mode; L.litSize = li.litSize; L.rawOff = li.rawOff; L.rleByte = li.rleByte; L.nStreams = li.nStreams; L.hufLog = S.hufLog;
-        for (int k = 0; k < 4; k++) { L.sOff[k] = li.sOff[k]; L.sLen[k] = li.sLen[k]; L.oOff[k] = li.oOff[k]; L.oCnt[k] = li.oCnt[k]; }
-        if (li.mode == 2) {
-            L.hufLitSize = li.litSize;
-            u32 const nE = 1u << S.hufLog;
-            for (u32 i = (u32)w.lane; i < nE; i += C::W) hufOut[i] = S.huf[i];
-            // a stream needs at least its end mark (HUF_decompress1X1 / BIT_initDStream: srcSize < 1 or a zero last byte is corruption)
-            for (u32 k = 0; k < li.nStreams; k++) {
-                L.sBits[k] = HUF_UNUSABLE;
-                if (li.sLen[k] < 1) { L.stB = E_corruption_detected; continue; }
-                u32 const last = blk[li.sOff[k] + li.sLen[k] - 1];
-                if (last == 0) { L.stB = E_corruption_detected; continue; }
-                L.sBits[k] = (li.sLen[k] - 1) * 8 + highbit32(last);
-            }
-        }
-        int nbSeq = 0;
-        size_t const hr = parse_seq_section(w, S, blk + lr, cSize - lr, dstCapacity, &nbSeq);
-        if (isErr(hr)) { L.stA2 = (u32)(0 - hr); break; }
-        if ((u32)nbSeq > FAST_MAXS) { L.mode = 0; break; }      // pathological: let the fused kernel deal with it
-        L.nbSeq = (u32)nbSeq; L.seqOff = (u32)(lr + hr); L.seqLen = (u32)(cSize - lr - hr);
-        if (nbSeq) {
-            L.logLL = S.fseLog[0]; L.logOF = S.fseLog[1]; L.logML = S.fseLog[2];
-            for (int t = 0; t < 3; t++) {
-                u32 const nE = 1u << S.fseLog[t];
-                u32* const out = fseOut + (t == 0 ? 0 : t == 1 ? FAST_FSE_OF : FAST_FSE_ML);
-                for (u32 i = (u32)w.lane; i < nE; i += C::W) {
-                    u32 const e = S.fse[t][i], sym = e >> 24;
-                    u32 const extra = t == 0 ? ZB_T.LL_bits[sym] : t == 1 ? sym : ZB_T.ML_bits[sym];
-                    out[i] = fse2_pack(e, extra);
-                }
-            }
-            // ZSTD_decompressSequences: BIT_initDStream fails on an empty stream or a zero last byte -> corruption_detected
-            if (L.seqLen < 1) { L.stC = E_corruption_detected; L.seqUnusable = 1; }
-            else {
-                u32 const last = blk[L.seqOff + L.seqLen - 1];
-                if (last == 0) { L.stC = E_corruption_detected; L.seqUnusable = 1; }
-                else L.seqBits = (L.seqLen - 1) * 8 + highbit32(last);
-            }
-        }
-    } while (0);
+        // refused: a 2^12-cell Huffman table (legal, never written by the reference) or a pathological sequence count
+        if (!prepare_block(w, S, src, (u32)ref, (u32)(ref >> 32), fh.blockSizeMax, dstCapacity, FAST_HUF_LOG, L, hufOut, fseOut)) L.mode = 0;
+    }
     w.sync();
     if (w.lane == 0) *d = L;
     w.sync();
@@ -366,7 +397,7 @@ struct HufChain {
 
 // host / emulator form of stage B: stream k of one frame
 ZB_HDN void dec_huf(DecDesc* d, int k, const u8* blk, const u16* huf, u8* lit) {
-    if (d->mode != 1 || d->stA1 || d->litMode != 2 || k >= (int)d->nStreams || d->sBits[k] == HUF_UNUSABLE) return;
+    if (d->mode != 1 || d->stA1 || d->litMode != 2 || k >= (int)d->nStreams || d->sBits[k] == NO_END_MARK) return;
     MemWords ws; ws.g.set(blk + d->sOff[k]);
     HufChain H;
     H.begin(ws, ws.g.floorBit, d->sBits[k], lit + d->oOff[k], d->oCnt[k]);

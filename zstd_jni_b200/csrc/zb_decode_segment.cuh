@@ -1,7 +1,8 @@
 // zb_decode_segment.cuh -- decoder for one frame of many blocks, a segment (a run of whole blocks) at a time, every stage parallel
 // over the blocks of the segment or over its output bytes (kernels k_seg_* in zb_capi.cu):
 //
-//   A  seg_prepare  warp / block     literal and sequence section headers, the tables the block describes -> HBM, stream geometry
+//   A  seg_prepare  warp / block     prepare_block (zb_decode_fast.cuh): literal and sequence section headers, the tables the block
+//                                    describes -> HBM, stream geometry
 //   B  seg_tables   one thread       in block order: the earlier block (or the carried state) whose table a repeating block reuses
 //   C  dec_huf      thread / stream  Huffman streams -> the block's literal buffer (zb_decode_fast.cuh)
 //      seg_seq      thread / block   sequence stream -> lengths and raw offset selectors, and the block's repcode summary
@@ -54,7 +55,7 @@ ZB_HD void rep_step_sym(RepSym* r, u32 idx, u32 v) {
 struct SegBlock {
     DecDesc d;           // as in the staged decoder; blockOff relative to the frame, mode 1 compressed / 2 raw / 3 rle
     u32 litType;         // literals block type of a compressed block (3: the previous Huffman table again)
-    u32 seqModes;        // symbol compression modes byte (a field of 3: the previous table again), 0 without sequences
+    u32 fseRepeat;       // bit t: FSE table t (LL, OF, ML) is the previous one again
     u32 hufSrc, fseSrc[3];    // segment block whose table the block uses, or SEG_CARRY
     u32 bad;             // the frame goes to the fused decoder
     u32 regen;
@@ -77,86 +78,29 @@ struct SegCarry {
 // The largest window the segment decoder takes (the default windowLogMax): larger ones stay with the fused decoder.
 constexpr u64 SEG_WINDOW_MAX = 1ull << 27;
 
-// Host side: the blocks of an item that is exactly one frame of more than one block -- magic number, no dictionary, a window of at most
-// SEG_WINDOW_MAX, every block inside the item, the checksum (when the frame has one) its last four bytes.  Returns the number of blocks
-// (0: the item is not such a frame); refs[k] = offset of block k's header | that header << 32, *xxh = the stored checksum.
+// Host side: the blocks of an item the segment decoder takes, one frame (frame_walk) of more than one block with a window of at most
+// SEG_WINDOW_MAX.  Returns the number of blocks, 0 for any other item.
 ZB_HDN u32 seg_walk(const u8* src, size_t size, FrameHeader* fh, u64* refs, u32* xxh) {
-    if (size < 9 || size > 0xFFFFFFFFu || load32(src) != MAGIC) return 0;
-    if (read_frame_header(fh, src, size) != 0 || fh->skippable || fh->dictID || fh->windowSize > SEG_WINDOW_MAX) return 0;
-    size_t pos = fh->headerSize; u32 n = 0;
-    for (;;) {
-        if (size - pos < 3) return 0;
-        u32 const bh = load24(src + pos), type = (bh >> 1) & 3;
-        size_t const cSize = type == 1 ? 1 : bh >> 3;
-        if (type == 3 || cSize > size - pos - 3) return 0;
-        if (refs) refs[n] = (u64)pos | ((u64)bh << 32);
-        n++; pos += 3 + cSize;
-        if (bh & 1) break;
-    }
-    if (size - pos != (fh->checksum ? 4u : 0u) || n < 2) return 0;
-    *xxh = fh->checksum ? load32(src + pos) : 0;
-    return n;
+    u32 const n = frame_walk(src, size, fh, 0xFFFFFFFFu, refs, xxh);
+    return n >= 2 && fh->windowSize <= SEG_WINDOW_MAX ? n : 0;
 }
 
 // ---------------------------------------------------------------------------------------- stage A
-// `bh` = the block header; the block's content starts at frame + off + 3.
+// `bh` = the block header, at frame + off.  The fused decoder takes the frame when a block is refused or has a nonzero stage status.
 template <class C>
 ZB_HDN void seg_prepare(const C& w, DecShared& S, const u8* frame, u32 off, u32 bh, u32 blockSizeMax, SegBlock* b, u16* hufOut, u32* fseOut) {
     SegBlock B;
     memset(&B, 0, sizeof B);
     DecDesc& L = B.d;
     L.outMax = 0xFFFFFFFFu;
-    u32 const type = (bh >> 1) & 3, cSize = bh >> 3;
-    L.blockOff = off + 3; L.cSize = type == 1 ? 1 : cSize;
-    do {
-        if (type == 0) { L.mode = 2; L.regen = cSize; break; }
-        if (type == 1) { L.mode = 3; L.regen = cSize; L.rleByte = frame[off + 3]; break; }
-        L.mode = 1;
-        if (type == 3 || cSize > blockSizeMax || cSize < 2) { B.bad = 1; break; }
-        const u8* const blk = frame + off + 3;
-        if (w.lane == 0) { S.litEntropy = 1; S.fseEntropy = 1; }      // repeats are resolved by seg_tables
-        w.sync();
-        B.litType = blk[0] & 3;
-        LitInfo li;
-        memset(&li, 0, sizeof li);
-        size_t const lr = parse_literals(w, S, blk, cSize, blockSizeMax, blockSizeMax, &li);
-        if (isErr(lr)) { B.bad = 1; break; }
-        L.litMode = li.mode; L.litSize = li.litSize; L.rawOff = li.rawOff; L.rleByte = li.rleByte; L.nStreams = li.nStreams;
-        for (int k = 0; k < 4; k++) { L.sOff[k] = li.sOff[k]; L.sLen[k] = li.sLen[k]; L.oOff[k] = li.oOff[k]; L.oCnt[k] = li.oCnt[k]; }
-        if (li.mode == 2) {
-            if (B.litType == 2) {
-                L.hufLog = S.hufLog;
-                for (u32 i = (u32)w.lane; i < (1u << S.hufLog); i += C::W) hufOut[i] = S.huf[i];
-            }
-            for (u32 k = 0; k < li.nStreams; k++) {
-                u32 const last = li.sLen[k] ? blk[li.sOff[k] + li.sLen[k] - 1] : 0;
-                if (last == 0) { B.bad = 1; break; }
-                L.sBits[k] = (li.sLen[k] - 1) * 8 + highbit32(last);
-            }
-            if (B.bad) break;
-        }
-        int nbSeq = 0;
-        size_t const hr = parse_seq_section(w, S, blk + lr, cSize - lr, 1, &nbSeq);
-        if (isErr(hr) || (u32)nbSeq > FAST_MAXS) { B.bad = 1; break; }
-        L.nbSeq = (u32)nbSeq; L.seqOff = (u32)(lr + hr); L.seqLen = (u32)(cSize - lr - hr);
-        if (nbSeq) {
-            u32 const b0 = blk[lr];
-            B.seqModes = blk[lr + (b0 < 0x80 ? 1 : b0 == 0xFF ? 3 : 2)];
-            u32* const logs[3] = { &L.logLL, &L.logOF, &L.logML };
-            for (int t = 0; t < 3; t++) {
-                if (((B.seqModes >> (6 - 2 * t)) & 3) == 3) continue;
-                *logs[t] = S.fseLog[t];
-                u32* const out = fseOut + (t == 0 ? 0 : t == 1 ? FAST_FSE_OF : FAST_FSE_ML);
-                for (u32 i = (u32)w.lane; i < (1u << S.fseLog[t]); i += C::W) {
-                    u32 const e = S.fse[t][i], sym = e >> 24;
-                    out[i] = fse2_pack(e, t == 0 ? ZB_T.LL_bits[sym] : t == 1 ? sym : ZB_T.ML_bits[sym]);
-                }
-            }
-            u32 const last = L.seqLen ? blk[L.seqOff + L.seqLen - 1] : 0;
-            if (last == 0) { B.bad = 1; break; }
-            L.seqBits = (L.seqLen - 1) * 8 + highbit32(last);
-        }
-    } while (0);
+    if (w.lane == 0) { S.litEntropy = 1; S.fseEntropy = 1; }      // repeats are resolved by seg_tables
+    w.sync();
+    bool const ok = prepare_block(w, S, frame, off, bh, blockSizeMax, blockSizeMax, HUF_TABLELOG_MAX, L, hufOut, fseOut);
+    B.bad = !ok || L.stA1 || L.stB || L.stA2 || L.stC;
+    if (!B.bad && L.mode == 1) {
+        B.litType = frame[off + 3] & 3;
+        for (int t = 0; t < 3 && L.nbSeq; t++) B.fseRepeat |= (S.fseMode[t] == 3 ? 1u : 0u) << t;
+    }
     w.sync();
     if (w.lane == 0) *b = B;
     w.sync();
@@ -181,11 +125,10 @@ ZB_HDN void seg_tables(SegBlock* blocks, u32 n, SegCarry* c, bool first, u64 cap
             B.hufSrc = huf; B.d.hufLog = huf == SEG_CARRY ? c->hufLog : blocks[huf].d.hufLog;
         } else if (B.litType == 2) huf = j;
         if (B.d.nbSeq) {
-            u32* const logs[3] = { &B.d.logLL, &B.d.logOF, &B.d.logML };
             for (int t = 0; t < 3; t++) {
-                if (((B.seqModes >> (6 - 2 * t)) & 3) == 3) {
+                if ((B.fseRepeat >> t) & 1) {
                     if (fse[t] == SEG_NONE) { c->bad = 1; break; }
-                    *logs[t] = fse[t] == SEG_CARRY ? c->fseLog[t] : (t == 0 ? blocks[fse[t]].d.logLL : t == 1 ? blocks[fse[t]].d.logOF : blocks[fse[t]].d.logML);
+                    B.d.fseLog[t] = fse[t] == SEG_CARRY ? c->fseLog[t] : blocks[fse[t]].d.fseLog[t];
                 } else fse[t] = j;
                 B.fseSrc[t] = fse[t];
             }
@@ -210,8 +153,7 @@ ZB_HDN void seg_seq(SegBlock* blocks, u32 j, const u8* frame, const u32* fseBase
     B.sumLL = 0; B.sumML = 0;
     if (B.d.mode != 1 || B.d.nbSeq == 0) return;
     const u32* t[3];
-    u32 const tOff[3] = { 0, FAST_FSE_OF, FAST_FSE_ML };
-    for (int k = 0; k < 3; k++) t[k] = (B.fseSrc[k] == SEG_CARRY ? c->fse : fseBase + (size_t)B.fseSrc[k] * FAST_FSE_ENTRIES) + tOff[k];
+    for (int k = 0; k < 3; k++) t[k] = (B.fseSrc[k] == SEG_CARRY ? c->fse : fseBase + (size_t)B.fseSrc[k] * FAST_FSE_ENTRIES) + fse_at(k);
     MemWords ws; ws.g.set(frame + B.d.blockOff + B.d.seqOff);
     SeqChain D;
     D.begin(ws, ws.g.floorBit, B.d.seqBits, B.d.logLL, B.d.logOF, B.d.logML, B.d.nbSeq);
@@ -274,12 +216,11 @@ ZB_HD void seg_carry_tables(const C& w, const SegBlock* blocks, const u16* hufBa
         for (u32 i = (u32)w.lane; i < SEG_HUF_ENTRIES; i += C::W) c->huf[i] = hufBase[(size_t)j * SEG_HUF_ENTRIES + i];
         if (w.lane == 0) { c->hufLog = blocks[j].d.hufLog; c->hasHuf = 1; }
     }
-    u32 const tOff[3] = { 0, FAST_FSE_OF, FAST_FSE_ML }, tLen[3] = { 512, 256, 512 };
     for (int t = 0; t < 3; t++) {
         if (c->nextFse[t] >= SEG_NONE) continue;
         u32 const j = c->nextFse[t];
-        for (u32 i = (u32)w.lane; i < tLen[t]; i += C::W) c->fse[tOff[t] + i] = fseBase[(size_t)j * FAST_FSE_ENTRIES + tOff[t] + i];
-        if (w.lane == 0) { c->fseLog[t] = t == 0 ? blocks[j].d.logLL : t == 1 ? blocks[j].d.logOF : blocks[j].d.logML; c->hasFse = 1; }
+        for (u32 i = fse_at(t) + (u32)w.lane; i < fse_at(t + 1); i += C::W) c->fse[i] = fseBase[(size_t)j * FAST_FSE_ENTRIES + i];
+        if (w.lane == 0) { c->fseLog[t] = blocks[j].d.fseLog[t]; c->hasFse = 1; }
     }
     w.sync();
 }
