@@ -189,6 +189,28 @@ ZSTDB200_API unsigned long long zstdb200_kernel_launches(const zstdb200_ctx* ctx
 /* frames of many blocks that zstdb200_decompress_batch gave to the segment decoder: regenerated there (deferred = 0), or handed to
  * the fused kernel because the segment decoder could not vouch for them (deferred = 1: corrupted, short of capacity, wrong checksum) */
 ZSTDB200_API unsigned long long zstdb200_segment_frames(const zstdb200_ctx* ctx, int deferred);
+
+/* Frame stream: one frame of many blocks decoded segment by segment as its blocks arrive, in memory that does not depend on the
+ * frame's size.  The handle keeps the frame's last window on the device (a ring of a power-of-two size, at least the window plus one
+ * segment's output) with the carried decoder state, and pinned host staging for at most one segment of input and one of output; each
+ * call borrows the segment workspace of the context it is given.
+ *   open:   parses the frame header at src (magicless: ZSTD_f_zstd1_magicless) and returns the bytes it took, or an error code:
+ *           srcSize_wrong when the header is not complete, frameParameter_windowTooLarge beyond windowMax, dictionary_wrong for a
+ *           frame that names a dictionary, parameter_unsupported for a skippable frame.  *fs receives the handle.
+ *   decode: takes bytes from src[*srcPos, srcSize) -- block headers, blocks, the checksum -- decodes a segment whenever
+ *           zstdb200_fstream_blocks(ctx) blocks or the last block are staged, and writes what it regenerated to dst[*dstPos,
+ *           dstCapacity), keeping the rest staged.  Returns 0 when the frame is done and handed out (the bytes after it are not
+ *           taken), 1 when it wants more input or more room, or an error code.  Bytes of earlier segments stay handed out.
+ *   stats:  0 segments regenerated by the segment decoder, 1 segments decoded on the fused decoder's resume entry (doubtful
+ *           segments, or every segment with dec_pipeline 0), 2 bytes of input and output the handle holds on the host. */
+typedef struct zstdb200_fstream_s zstdb200_fstream;
+ZSTDB200_API unsigned zstdb200_fstream_blocks(const zstdb200_ctx* ctx);      /* blocks per segment (dec_segment_blocks) */
+ZSTDB200_API size_t zstdb200_fstream_open(zstdb200_ctx* ctx, const void* src, size_t srcSize, int magicless, unsigned long long windowMax,
+                                          zstdb200_fstream** fs);
+ZSTDB200_API size_t zstdb200_fstream_decode(zstdb200_ctx* ctx, zstdb200_fstream* fs, const void* src, size_t srcSize, size_t* srcPos,
+                                            void* dst, size_t dstCapacity, size_t* dstPos);
+ZSTDB200_API unsigned long long zstdb200_fstream_stats(const zstdb200_fstream* fs, int what);
+ZSTDB200_API void zstdb200_fstream_free(zstdb200_fstream* fs);
 /* with option "timing" = 1 every kernel launch is bracketed by CUDA events on its stream; this returns the averages
  * since the previous call as "name:ms:count;..." (synchronises).  Used by bench.py for the roofline line. */
 ZSTDB200_API size_t zstdb200_kernel_times(zstdb200_ctx* ctx, char* buf, size_t cap);

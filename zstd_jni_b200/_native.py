@@ -108,6 +108,11 @@ def lib() -> C.CDLL:
     sig("zstdb200_set_option", i, vp, C.c_char_p, C.c_longlong)
     sig("zstdb200_kernel_launches", C.c_ulonglong, vp)
     sig("zstdb200_segment_frames", C.c_ulonglong, vp, i)
+    sig("zstdb200_fstream_blocks", C.c_uint, vp)
+    sig("zstdb200_fstream_open", sz, vp, vp, sz, i, C.c_ulonglong, C.POINTER(vp))
+    sig("zstdb200_fstream_decode", sz, vp, vp, vp, sz, c_size_p, vp, sz, c_size_p)
+    sig("zstdb200_fstream_stats", C.c_ulonglong, vp, i)
+    sig("zstdb200_fstream_free", None, vp)
     sig("zstdb200_kernel_times", sz, vp, C.c_char_p, sz)
     sig("zstdb200_compress_chunks", sz, vp, i, vp, sz, sz, vp, sz, c_size_p, c_size_p)
     sig("zstdb200_decompress_frames", sz, vp, vp, c_size_p, sz, vp, sz, c_size_p)

@@ -12,8 +12,13 @@
 //   D  seg_fill     warp / block     link map: every output byte of the segment is a final byte or the segment byte it copies
 //      seg_jump     thread / byte    pointer jumping on the link map, in place, until every byte is final; the bytes -> dst
 //
-// Between segments the frame carries its output position, the repcode history and its last Huffman / FSE tables (SegCarry).  The
-// whole frame's output lies in dst, so copies reach back to the frame start, as in the fused decoder.
+// Between segments the frame carries its output position, the repcode history and its last Huffman / FSE tables (SegCarry); nothing
+// of it points into the input, so every segment may be read from its own staged copy.  Copies that reach before the segment read the
+// history: the frame's output in dst (batch items, mask ~0), or a ring of a power-of-two size that keeps the last window of a streamed
+// frame (zstdb200_fstream_*), at frame position & mask.
+//
+// seg_resume is the fused decoder entered at a block boundary: from the carried state and a linear copy of the history it decodes one
+// segment's blocks and leaves the carried state as the segment decoder would, so the next segment may go either way.
 //
 // The segment path decides no error itself.  Whatever the fused decoder could reject -- a stage status, a table repeated before any
 // block described it, a block regenerating more than blockSizeMax, an offset reaching before the frame, output beyond the capacity or
@@ -230,9 +235,10 @@ ZB_HD void seg_carry_tables(const C& w, const SegBlock* blocks, const u16* hufBa
 // the segment are final, a match byte inside the segment names the byte it copies -- for a match that overlaps itself, the byte of its
 // first period, so that a run is one link deep.  Sequences go 32 at a time, their bytes are spread over the lanes.
 struct SegRec { u64 o, md; u32 ls, off; };
+// `hist`: the output before the segment, frame position p at hist[p & mask]; an offset beyond `window` marks the frame bad.
 template <class C>
 ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const u8* frame, const u8* lit, const u64* seqs, const u32* offs,
-                     const u8* dst, u64 segStart, u32* link, SegCarry* c) {
+                     const u8* hist, u64 mask, u64 window, u64 segStart, u32* link, SegCarry* c) {
     SegBlock const& B = blocks[j];
     u64 const base = B.out;
     auto put = [&](u64 p, u32 v) { link[p - segStart] = v; };
@@ -251,7 +257,7 @@ ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const
         u32 const ll = (u32)(q & 0x3FFFF), ml = (u32)((q >> 18) & 0x3FFFF), off = i < B.d.nbSeq ? offs[i] : 0;
         u64 const o = op + w.exscan(ll + ml);
         u32 const ls = lp + w.exscan(ll);
-        bool const bad = i < B.d.nbSeq && (u64)off > o + ll;        // the copy would start before the frame (ZSTD_execSequence :1034)
+        bool const bad = i < B.d.nbSeq && ((u64)off > o + ll || off > window);     // before the frame (ZSTD_execSequence :1034) or the window
         if (w.ballot(bad)) { if (w.lane == 0) c->bad = 1; return; }
         SegRec r; r.o = o; r.md = o + ll; r.ls = ls; r.off = off;
         R[w.lane] = r;
@@ -267,7 +273,7 @@ ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const
             if (p < e.md) v = SEG_FINAL | (rle ? B.d.rleByte : L[e.ls + (u32)(p - e.o)]);
             else {
                 u64 const src = e.md - e.off + (p - e.md) % e.off;
-                v = src < segStart ? SEG_FINAL | dst[src] : (u32)(src - segStart);
+                v = src < segStart ? SEG_FINAL | hist[src & mask] : (u32)(src - segStart);
             }
             put(p, v);
         }
@@ -278,12 +284,96 @@ ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const
     w.sync();
 }
 
+// The history is the frame's whole output in dst.
+template <class C>
+ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const u8* frame, const u8* lit, const u64* seqs, const u32* offs,
+                     const u8* dst, u64 segStart, u32* link, SegCarry* c) {
+    seg_fill(w, R, blocks, j, frame, lit, seqs, offs, dst, ~0ull, ~0ull, segStart, link, c);
+}
+
 // Segment byte p: follows its links, shortening its own entry on the way (others that reach it later jump further), until a final
 // byte.  Every link points to an earlier byte, so the walk ends; an entry only ever changes to another entry on its own chain.
 ZB_HD u8 seg_jump(volatile u32* link, u32 p) {
     u32 v = link[p];
     while (!(v & SEG_FINAL)) { v = link[v]; link[p] = v; }
     return (u8)v;
+}
+
+
+// ---------------------------------------------------------------------------------------- resume
+// The fused decoder (zb_decode.cuh) from a block boundary: the n blocks at in + (u32)refs[j] (headers refs[j] >> 32) of the segment that
+// starts at frame position c->pos, written to out, with the history hist[0, out - hist) right before it -- offsets reaching before
+// hist are corruption, as they are before the frame start.  The repcodes and the last tables come from the carried state and go back
+// to it; the FSE cells are carried in the staged format (fse2_pack), which keeps the fields of the fused format.  Returns the bytes
+// written or the fused decoder's error code.
+ZB_HD u32 fse2_unpack(u32 e) { return ((e >> 16) & 0x1FFu) | (((e >> 8) & 0xFFu) << 16) | ((e >> 25) << 24); }
+template <class C>
+ZB_HDN size_t seg_resume(const C& w, DecShared& S, const u8* in, const u64* refs, u32 n, u32 blockSizeMax, const u8* hist, u8* out,
+                         size_t cap, u8* scratch, SegCarry* c) {
+    if (w.lane == 0) {
+        for (int s = 0; s < 3; s++) { S.rep[s] = c->rep[s]; S.fseLog[s] = c->fseLog[s]; }
+        S.litEntropy = c->hasHuf; S.fseEntropy = c->hasFse; S.hufLog = c->hufLog;
+    }
+    w.sync();
+    if (c->hasHuf) for (u32 i = (u32)w.lane; i < (1u << c->hufLog); i += C::W) S.huf[i] = c->huf[i];
+    if (c->hasFse)
+        for (int t = 0; t < 3; t++)
+            for (u32 i = (u32)w.lane; i < (1u << c->fseLog[t]); i += C::W) S.fse[t][i] = fse2_unpack(c->fse[fse_at(t) + i]);
+    w.sync();
+    size_t written = 0;
+    for (u32 j = 0; j < n; j++) {
+        u32 const bh = (u32)(refs[j] >> 32), type = (bh >> 1) & 3;
+        size_t const cSize = type == 1 ? 1 : bh >> 3;
+        const u8* const ip = in + (u32)refs[j] + 3;
+        size_t decoded;
+        if (type == 2) {
+            decoded = decode_block(w, S, hist, out + written, cap - written, ip, cSize, blockSizeMax, scratch);
+            if (isErr(decoded)) return decoded;
+        } else if (type == 0) {
+            if (cSize > cap - written) return ERR(E_dstSize_tooSmall);
+            for (size_t k = (size_t)w.lane; k < cSize; k += C::W) out[written + k] = ip[k];
+            decoded = cSize; w.sync();
+        } else if (type == 1) {
+            size_t const rl = bh >> 3;
+            if (rl > cap - written) return ERR(E_dstSize_tooSmall);
+            for (size_t k = (size_t)w.lane; k < rl; k += C::W) out[written + k] = ip[0];
+            decoded = rl; w.sync();
+        } else return ERR(E_corruption_detected);
+        written += decoded;
+    }
+    if (S.litEntropy) for (u32 i = (u32)w.lane; i < (1u << S.hufLog); i += C::W) c->huf[i] = S.huf[i];
+    if (S.fseEntropy)
+        for (int t = 0; t < 3; t++)
+            for (u32 i = (u32)w.lane; i < (1u << S.fseLog[t]); i += C::W) {
+                u32 const e = S.fse[t][i], sym = e >> 24;
+                c->fse[fse_at(t) + i] = fse2_pack(e, t == 0 ? ZB_T.LL_bits[sym] : t == 1 ? sym : ZB_T.ML_bits[sym]);
+            }
+    w.sync();
+    if (w.lane == 0) {
+        for (int s = 0; s < 3; s++) { c->rep[s] = S.rep[s]; c->fseLog[s] = S.fseLog[s]; }
+        c->hasHuf = S.litEntropy; c->hasFse = S.fseEntropy; c->hufLog = S.hufLog; c->pos += written;
+    }
+    w.sync();
+    return written;
+}
+
+// A streamed frame's block the reference's streaming decoder rejects from its 3-byte header `bh` alone: a reserved type, or more than
+// blockSizeMax bytes of block content or of RLE output (ZSTD_decompressContinue, corruption_detected).
+ZB_HD bool stream_block_error(u32 bh, u32 blockSizeMax) {
+    return ((bh >> 1) & 3) == 3 || (bh >> 3) > blockSizeMax;
+}
+
+// The frame stream's result of a segment on the resume entry.  The fused decoder stops a damaged block at blockSizeMax + 32 bytes of
+// output with dstSize_tooSmall, as the reference's one-shot decoder does; the reference's streaming decoder decodes into a buffer with
+// room beyond the block and rejects the block at its end with corruption_detected (ZSTD_decompressContinue :1367).  With the resume
+// entry's room, dstSize_tooSmall can only be that limit, so the stream reports the streaming decoder's code.
+ZB_HD size_t stream_resume_result(size_t r) { return r == ERR(E_dstSize_tooSmall) ? ERR(E_corruption_detected) : r; }
+
+// The carried state at the start of a frame, before its first segment (what seg_tables sets up for `first`).
+ZB_HD void seg_carry_init(SegCarry* c, u64 cap) {
+    c->pos = 0; c->cap = cap; c->bad = 0; c->hasHuf = 0; c->hasFse = 0; c->hufLog = 0;
+    c->rep[0] = 1; c->rep[1] = 4; c->rep[2] = 8;
+    for (int t = 0; t < 3; t++) c->fseLog[t] = 0;
 }
 
 }  // namespace zb

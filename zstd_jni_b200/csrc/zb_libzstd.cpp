@@ -41,7 +41,8 @@ struct PooledCtx {
 };
 
 // host-side frame walks (no GPU needed): same parsers as the kernels, host instantiation of the headers
-// `missing` (optional): when the frame is cut short (srcSize_wrong), the least number of further bytes that lets the walk advance
+// `missing` (optional): when the frame is cut short (srcSize_wrong), the least number of further bytes that lets the walk advance;
+// *nbBlocks then holds the whole blocks present
 size_t host_find_frame_size(const u8* src, size_t srcSize, size_t* nbBlocks, FrameHeader* fhOut, u32 magicless = 0, size_t* missing = nullptr) {
     if (missing) *missing = 1;
     // inputs may be unaligned / tiny: copy the few bytes we look at into an aligned scratch when needed
@@ -56,6 +57,7 @@ size_t host_find_frame_size(const u8* src, size_t srcSize, size_t* nbBlocks, Fra
     if (fh.skippable) { if ((u64)fh.skipLen + 8 > srcSize) { if (missing) *missing = (size_t)((u64)fh.skipLen + 8 - srcSize); return ERR(E_srcSize_wrong); } if (nbBlocks) *nbBlocks = 0; return 8 + (size_t)fh.skipLen; }
     size_t pos = fh.headerSize, blocks = 0;
     for (;;) {
+        if (nbBlocks) *nbBlocks = blocks;
         if (srcSize - pos < 3) { if (missing) *missing = 3 - (srcSize - pos); return ERR(E_srcSize_wrong); }
         u32 const bh = (u32)src[pos] | ((u32)src[pos + 1] << 8) | ((u32)src[pos + 2] << 16);
         u32 const type = (bh >> 1) & 3; size_t cSize = bh >> 3;
@@ -152,6 +154,10 @@ struct ZSTD_DCtx_s {
     RawBuf inBuf;               // bytes of the frame being collected
     RawBuf outBuf;              // regenerated bytes not yet handed out
     size_t outPos = 0;
+    zstdb200_fstream* fs = nullptr;      // a frame of more blocks than one segment, streamed segment by segment
+    u32 segBlocks = 0;                   // blocks per segment of the batch contexts (0: not asked yet)
+    void end_frame_stream() { zstdb200_fstream_free(fs); fs = nullptr; }
+    ~ZSTD_DCtx_s() { end_frame_stream(); }
 };
 
 extern "C" {
@@ -209,14 +215,14 @@ size_t ZSTD_CCtx_reset(ZSTD_CCtx* c, ZSTD_ResetDirective reset) {
 }
 size_t ZSTD_DCtx_reset(ZSTD_DCtx* d, ZSTD_ResetDirective reset) {
     if (!d) return ERR(E_GENERIC);
-    if (reset != ZSTD_reset_parameters) { d->inBuf.clear(); d->outBuf.clear(); d->outPos = 0; }
+    if (reset != ZSTD_reset_parameters) { d->inBuf.clear(); d->outBuf.clear(); d->outPos = 0; d->end_frame_stream(); }
     if (reset != ZSTD_reset_session_only) { d->format = 0; d->maxWindowSize = (1ull << 27) + 1; }
     return 0;
 }
 // N/jni_zstd.c:403 (setDecompressionLongMax), :413-414 (setDecompressionMagicless); ZSTD_dParam_getBounds, N/decompress/zstd_decompress.c:1838-1878
 size_t ZSTD_DCtx_setParameter(ZSTD_DCtx* d, ZSTD_dParameter param, int value) {
     if (!d) return ERR(E_GENERIC);
-    if (!d->inBuf.empty() || d->outPos < d->outBuf.size()) return ERR(E_stage_wrong);
+    if (!d->inBuf.empty() || d->outPos < d->outBuf.size() || d->fs) return ERR(E_stage_wrong);
     switch (param) {
     case ZSTD_d_windowLogMax:
         if (value == 0) value = 27;
@@ -450,6 +456,9 @@ size_t ZSTD_initDStream(ZSTD_DStream* z) { if (!z) return ERR(E_GENERIC); ZSTD_D
 // Decoding side.  Whole frames are decoded, as many as the offered input holds and one batch takes; only a frame cut by the end
 // of the input is copied aside until the rest arrives.  Memory is bounded by what the blocks PRESENT in the input can regenerate
 // (blocks x blockSizeMax): a frame header promising more than that is corruption, it never sizes an allocation.
+// A frame of more blocks than one segment (zstdb200_fstream_blocks) goes to a frame stream instead, whether it is present whole or cut
+// by the end of the input: its segments are decoded as their blocks arrive and handed out one after the other, in memory bounded by
+// its window and one segment.
 static size_t dstream_frame_bound(const FrameHeader& fh, size_t blocks, u64* bound) {
     if (fh.skippable) { *bound = 0; return 0; }
     u64 const byBlocks = (u64)blocks * fh.blockSizeMax;
@@ -470,6 +479,23 @@ static size_t decompress_stream(ZSTD_DStream* d, ZSTD_outBuffer* out, ZSTD_inBuf
             if (k) { memcpy((u8*)out->dst + out->pos, d->outBuf.data() + d->outPos, k); out->pos += k; d->outPos += k; }
             if (d->outPos < d->outBuf.size()) return 1;   // more to flush
             d->outBuf.clear(); d->outPos = 0; }
+        // a frame stream in progress takes the bytes put aside, then the caller's
+        if (d->fs) {
+            PooledCtx g(d->format ? FRAME_MAGICLESS : 0u, CParams{});
+            if (!g.ok) return ERR(E_GENERIC);
+            size_t r = 1;
+            if (!d->inBuf.empty()) {
+                size_t ip = 0;
+                r = zstdb200_fstream_decode(g.c, d->fs, d->inBuf.data(), d->inBuf.size(), &ip, out->dst, out->size, &out->pos);
+                d->inBuf.erase_front(ip);
+            }
+            if (r == 1 && d->inBuf.empty()) r = zstdb200_fstream_decode(g.c, d->fs, in->src, in->size, &in->pos, out->dst, out->size, &out->pos);
+            if (r == 1) return 1;
+            d->end_frame_stream();
+            if (isErr(r)) return r;
+            if (d->inBuf.empty() && in->pos == in->size) return 0;
+            continue;                            // the frame is done: the bytes after it
+        }
         // where the next frames are: the bytes put aside, or the caller's buffer
         bool const aside = !d->inBuf.empty();
         if (aside && in->pos < in->size) {       // complete the frame that was cut: take what its header / blocks say is missing
@@ -490,6 +516,13 @@ static size_t decompress_stream(ZSTD_DStream* d, ZSTD_outBuffer* out, ZSTD_inBuf
         }
         const u8* const base = aside ? d->inBuf.data() : (const u8*)in->src + in->pos;
         size_t const have = aside ? d->inBuf.size() : in->size - in->pos;
+        // a frame of more blocks than one segment, present whole or cut, that is the first here: it becomes the frame stream
+        auto streams = [&](const FrameHeader& fh, size_t blocks) {
+            if (blocks <= 1 || fh.skippable || fh.windowSize > d->maxWindowSize) return false;      // (fh is set once blocks are)
+            if (!d->segBlocks) { PooledCtx g(0u, CParams{}); if (!g.ok) return false; d->segBlocks = zstdb200_fstream_blocks(g.c); }
+            return blocks > d->segBlocks;
+        };
+        bool stream = false;
         // walk the whole frames present
         std::vector<size_t> fsz, cap, slot;
         size_t used = 0; u64 outTotal = 0;
@@ -497,6 +530,7 @@ static size_t decompress_stream(ZSTD_DStream* d, ZSTD_outBuffer* out, ZSTD_inBuf
             if (have - used < minHdr) break;
             FrameHeader fh; size_t blocks = 0;
             size_t const fs = host_find_frame_size(base + used, have - used, &blocks, &fh, (u32)d->format);
+            if ((!isErr(fs) || fs == ERR(E_srcSize_wrong)) && streams(fh, blocks)) { stream = fsz.empty(); break; }
             if (isErr(fs)) { if (fs == ERR(E_srcSize_wrong)) break; if (fsz.empty()) return fs; break; }      // a later frame's error surfaces when it is first
             u64 bound = 0;
             {   size_t const r = dstream_frame_bound(fh, blocks, &bound); if (isErr(r)) { if (fsz.empty()) return r; break; } }
@@ -506,6 +540,14 @@ static size_t decompress_stream(ZSTD_DStream* d, ZSTD_outBuffer* out, ZSTD_inBuf
                 break;
             }
             fsz.push_back(fs); cap.push_back((size_t)bound); slot.push_back((size_t)bound); used += fs; outTotal += bound;
+        }
+        if (stream) {
+            PooledCtx g(d->format ? FRAME_MAGICLESS : 0u, CParams{});
+            if (!g.ok) return ERR(E_GENERIC);
+            size_t const h = zstdb200_fstream_open(g.c, base, have, d->format, d->maxWindowSize, &d->fs);
+            if (isErr(h)) return h;
+            if (aside) d->inBuf.erase_front(h); else in->pos += h;
+            continue;
         }
         if (!fsz.empty()) {
             // straight into the caller's buffer when everything fits there, else through outBuf
