@@ -108,6 +108,7 @@ def lib() -> C.CDLL:
     sig("zstdb200_set_option", i, vp, C.c_char_p, C.c_longlong)
     sig("zstdb200_kernel_launches", C.c_ulonglong, vp)
     sig("zstdb200_segment_frames", C.c_ulonglong, vp, i)
+    sig("zstdb200_split_items", C.c_ulonglong, vp, i)
     sig("zstdb200_fstream_blocks", C.c_uint, vp)
     sig("zstdb200_fstream_open", sz, vp, vp, sz, i, C.c_ulonglong, C.POINTER(vp))
     sig("zstdb200_fstream_decode", sz, vp, vp, vp, sz, c_size_p, vp, sz, c_size_p)

@@ -167,25 +167,63 @@ ZB_HD u64 peek_bits(const u8* p, i64 lo, u32 n) {
 }
 
 // ---------------------------------------------------------------- XXH64
-// published xxHash64 (N/common/xxhash.h), serial; only used when the frame asks for it.
+// published xxHash64 (N/common/xxhash.h); only used when the frame asks for it.  The pieces are shared by the serial form and the
+// warp-cooperative one.
 ZB_HD u64 rotl64(u64 x, int r) { return (x << r) | (x >> (64 - r)); }
-ZB_HDN u64 xxh64(const u8* p, size_t len) {
-    constexpr u64 P1 = 0x9E3779B185EBCA87ULL, P2 = 0xC2B2AE3D27D4EB4FULL, P3 = 0x165667B19E3779F9ULL, P4 = 0x85EBCA77C2B2AE63ULL, P5 = 0x27D4EB2F165667C5ULL;
-    const u8* const end = p + len; u64 h;
-    auto rnd = [&](u64 acc, u64 in) { acc += in * P2; acc = rotl64(acc, 31); return acc * P1; };
-    auto mrg = [&](u64 acc, u64 v) { v = rnd(0, v); acc ^= v; return acc * P1 + P4; };
-    if (len >= 32) {
-        u64 v1 = P1 + P2, v2 = P2, v3 = 0, v4 = 0 - P1;
-        do { v1 = rnd(v1, load64(p)); v2 = rnd(v2, load64(p + 8)); v3 = rnd(v3, load64(p + 16)); v4 = rnd(v4, load64(p + 24)); p += 32; } while (p + 32 <= end);
-        h = rotl64(v1, 1) + rotl64(v2, 7) + rotl64(v3, 12) + rotl64(v4, 18);
-        h = mrg(h, v1); h = mrg(h, v2); h = mrg(h, v3); h = mrg(h, v4);
-    } else h = P5;
-    h += (u64)len;
-    while (p + 8 <= end) { h ^= rnd(0, load64_n(p, 8)); h = rotl64(h, 27) * P1 + P4; p += 8; }
-    if (p + 4 <= end) { h ^= (u64)load32(p) * P1; h = rotl64(h, 23) * P2 + P3; p += 4; }
-    while (p < end) { h ^= (*p++) * P5; h = rotl64(h, 11) * P1; }
-    h ^= h >> 33; h *= P2; h ^= h >> 29; h *= P3; h ^= h >> 32;
+constexpr u64 XXH_P1 = 0x9E3779B185EBCA87ULL, XXH_P2 = 0xC2B2AE3D27D4EB4FULL, XXH_P3 = 0x165667B19E3779F9ULL, XXH_P4 = 0x85EBCA77C2B2AE63ULL,
+              XXH_P5 = 0x27D4EB2F165667C5ULL;
+// the seed-0 start of accumulator a (0..3)
+ZB_HD u64 xxh_acc0(u32 a) { return a == 0 ? XXH_P1 + XXH_P2 : a == 1 ? XXH_P2 : a == 2 ? 0 : 0 - XXH_P1; }
+ZB_HD u64 xxh_round(u64 acc, u64 in) { acc += in * XXH_P2; acc = rotl64(acc, 31); return acc * XXH_P1; }
+// the four accumulators after the last whole 32-byte stripe -> the hash state before the length is added
+ZB_HD u64 xxh_converge(u64 v1, u64 v2, u64 v3, u64 v4) {
+    auto mrg = [](u64 acc, u64 v) { acc ^= xxh_round(0, v); return acc * XXH_P1 + XXH_P4; };
+    u64 h = rotl64(v1, 1) + rotl64(v2, 7) + rotl64(v3, 12) + rotl64(v4, 18);
+    h = mrg(h, v1); h = mrg(h, v2); h = mrg(h, v3); h = mrg(h, v4);
     return h;
+}
+// the last len % 32 bytes [p, end) and the avalanche; h = the state after the stripes plus the total length
+ZB_HD u64 xxh_finish(u64 h, const u8* p, const u8* end) {
+    while (p + 8 <= end) { h ^= xxh_round(0, load64_n(p, 8)); h = rotl64(h, 27) * XXH_P1 + XXH_P4; p += 8; }
+    if (p + 4 <= end) { h ^= (u64)load32(p) * XXH_P1; h = rotl64(h, 23) * XXH_P2 + XXH_P3; p += 4; }
+    while (p < end) { h ^= (*p++) * XXH_P5; h = rotl64(h, 11) * XXH_P1; }
+    h ^= h >> 33; h *= XXH_P2; h ^= h >> 29; h *= XXH_P3; h ^= h >> 32;
+    return h;
+}
+// serial: one thread
+ZB_HDN u64 xxh64(const u8* p, size_t len) {
+    const u8* const end = p + len; u64 h;
+    if (len >= 32) {
+        u64 v1 = xxh_acc0(0), v2 = xxh_acc0(1), v3 = xxh_acc0(2), v4 = xxh_acc0(3);
+        do { v1 = xxh_round(v1, load64(p)); v2 = xxh_round(v2, load64(p + 8)); v3 = xxh_round(v3, load64(p + 16)); v4 = xxh_round(v4, load64(p + 24)); p += 32; }
+        while (p + 32 <= end);
+        h = xxh_converge(v1, v2, v3, v4);
+    } else h = XXH_P5;
+    return xxh_finish(h + (u64)len, p, end);
+}
+// Warp-cooperative, the same hash; every lane returns it.  Each round the warp reads W x 8 bytes (W / 4 stripes) with one 8-byte load
+// per lane, all of them issued before any is needed; lanes 0..3 then run the four accumulators over the round's words, which they take
+// from the other lanes by shuffles.  Lane 0 converges the accumulators and hashes the tail.  A warp of fewer than four lanes hashes
+// serially.
+template <class C>
+ZB_HD u64 xxh64_warp(const C& w, const u8* p, size_t len) {
+    if (C::W < 4) return xxh64(p, len);
+    constexpr u32 SPR = C::W >= 4 ? (u32)C::W / 4 : 1u;      // stripes per round
+    size_t const stripes = len / 32;
+    u32 const a = (u32)w.lane & 3;
+    u64 v = xxh_acc0(a);
+    for (size_t s0 = 0; s0 < stripes; s0 += SPR) {
+        u32 const ns = stripes - s0 < SPR ? (u32)(stripes - s0) : SPR;      // uniform
+        u64 const word = (u32)w.lane < 4 * ns ? load64(p + 32 * s0 + 8 * (u32)w.lane) : 0;
+        for (u32 j = 0; j < ns; j++) {
+            u64 const in = w.shfl(word, (int)(4 * j + a));
+            v = xxh_round(v, in);
+        }
+    }
+    u64 h = 0;
+    u64 const v2 = w.shfl(v, 1), v3 = w.shfl(v, 2), v4 = w.shfl(v, 3);
+    if (w.lane == 0) h = xxh_finish((stripes ? xxh_converge(v, v2, v3, v4) : XXH_P5) + (u64)len, p + 32 * stripes, p + len);
+    return w.bcast(h);
 }
 
 // ---- backward bit reader of ONE thread, all in 32-bit registers.

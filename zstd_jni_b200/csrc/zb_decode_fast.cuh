@@ -16,10 +16,11 @@
 // plain byte array.  Their tables sit in shared memory, brought in by one bulk asynchronous copy
 // (cp.async.bulk + mbarrier) per table when a lane takes its next frame.
 //
-// An item is eligible when it is exactly one frame with one (last) block, carries its content size and no
-// checksum; everything else (multi-block, multi-frame, skippable, checksummed, > MAXS sequences, 2^12-cell Huffman
-// tables) is left to the fused kernel.  Results -- including the error code of corrupted input -- are identical to
-// the fused path: the stage statuses are combined in the order the fused decoder would have met the errors.
+// An item is eligible when it is exactly one frame with one (last) block and carries its content size; a checksum is
+// verified at the end of stage D by the warp (xxh64_warp).  Everything else (multi-block, skippable, > MAXS sequences,
+// 2^12-cell Huffman tables) is left to the fused kernel or the segment decoder; an item of several frames is cut into
+// its frames first (item_walk, zstdb200_decompress_batch).  Results -- including the error code of corrupted input --
+// are identical to the fused path: the stage statuses are combined in the order the fused decoder would have met the errors.
 //
 // Reference behaviour reproduced: see zb_decode.cuh (N/decompress/zstd_decompress_block.c:134-340,695-775,
 // 1001-1096,1229-1346,1615-1690; N/decompress/huf_decompress.c:574-698).
@@ -76,7 +77,9 @@ static_assert(sizeof(DecDesc) == 184 && offsetof(DecDesc, sBits) == 124 && offse
 // The blocks of an item that is exactly one frame of at most maxBlocks blocks: magic number, no dictionary, every block inside the item,
 // the checksum (when the frame has one) its last four bytes.  Returns the number of blocks (0: the item is not such a frame);
 // refs[k] = offset of block k's header | that header << 32 (refs may be null), *xxh = the stored checksum.
-ZB_HDN u32 frame_walk(const u8* src, size_t size, FrameHeader* fh, u32 maxBlocks, u64* refs, u32* xxh) {
+// With `end`, the frame only has to start the item: *end = its size (frames past 4 GiB are not taken).
+ZB_HDN u32 frame_walk(const u8* src, size_t size, FrameHeader* fh, u32 maxBlocks, u64* refs, u32* xxh, size_t* end = nullptr) {
+    if (end && size > 0xFFFFFFFFu) size = 0xFFFFFFFFu;
     if (size < 9 || size > 0xFFFFFFFFu || load32(src) != MAGIC) return 0;
     if (read_frame_header(fh, src, size) != 0 || fh->skippable || fh->dictID) return 0;
     size_t pos = fh->headerSize; u32 n = 0;
@@ -89,8 +92,44 @@ ZB_HDN u32 frame_walk(const u8* src, size_t size, FrameHeader* fh, u32 maxBlocks
         n++; pos += 3 + cSize;
         if (bh & 1) break;
     }
-    if (size - pos != (fh->checksum ? 4u : 0u)) return 0;
+    size_t const tail = fh->checksum ? 4u : 0u;
+    if (end ? size - pos < tail : size - pos != tail) return 0;
     *xxh = fh->checksum ? load32(src + pos) : 0;
+    if (end) *end = pos + tail;
+    return n;
+}
+
+// One frame of an item as item_walk lists it.
+struct ItemFrame { u64 srcOff, srcSize, contentSize; u32 nBlocks, checksum, hasContentSize, skippable; };
+
+// The frames of an item, for decoding them one by one: frame_walk for each zstd frame, read_frame_header for each skippable one (it
+// regenerates nothing).  Lists the frames walked from the item's start into out[0 .. outMax) (out may be null) and returns their number;
+// the walk stops where no whole frame follows.  *split: the item may be decoded frame by frame -- the walk covers it exactly, it has at
+// least two frames (skippable ones count), every zstd frame but the last declares its content size, and the declared sizes add up to
+// at most `capacity` (the last zstd frame, if it declares none, gets the rest).  Any other item is decoded whole.
+ZB_HDN u32 item_walk(const u8* src, size_t size, u64 capacity, ItemFrame* out, u32 outMax, bool* split) {
+    u32 n = 0; size_t pos = 0; u64 declared = 0;
+    bool sized = true, ok = true;      // sized: every zstd frame so far declares its content size
+    while (pos < size) {
+        ItemFrame f{}; FrameHeader fh;
+        f.srcOff = pos;
+        size_t const rest = size - pos;
+        if (rest >= 8 && (load32(src + pos) & 0xFFFFFFF0u) == 0x184D2A50u) {
+            if (read_frame_header(&fh, src + pos, rest) != 0 || (u64)fh.skipLen + 8 > rest) break;
+            f.srcSize = 8 + (u64)fh.skipLen; f.skippable = 1;
+        } else {
+            size_t end = 0; u32 xxh;
+            u32 const nb = frame_walk(src + pos, rest, &fh, 0xFFFFFFFFu, nullptr, &xxh, &end);
+            if (!nb) break;
+            if (!sized) ok = false;                  // a zstd frame after one without a content size
+            f.srcSize = end; f.nBlocks = nb; f.checksum = fh.checksum; f.hasContentSize = fh.hasContentSize; f.contentSize = fh.contentSize;
+            if (fh.hasContentSize) declared += fh.contentSize <= capacity ? fh.contentSize : capacity + 1;      // (no wrap)
+            else sized = false;
+        }
+        if (out && n < outMax) out[n] = f;
+        n++; pos += (size_t)f.srcSize;
+    }
+    *split = ok && pos == size && n >= 2 && declared <= capacity;
     return n;
 }
 
@@ -151,14 +190,14 @@ ZB_HD bool prepare_block(const C& w, DecShared& S, const u8* item, u32 off, u32 
     return true;
 }
 
-// The staged decoder takes an item that is one frame of one block, with its content size (at most one block) and no checksum.
-// All lanes of a warp; S is the warp's shared scratch; tables are copied out to hufOut / fseOut.
+// The staged decoder takes an item that is one frame of one block, with its content size (at most one block); dec_exec verifies the
+// checksum when the frame has one.  All lanes of a warp; S is the warp's shared scratch; tables are copied out to hufOut / fseOut.
 template <class C>
 ZB_HDN void dec_prepare(const C& w, DecShared& S, const u8* src, size_t srcSize, size_t dstCapacity, DecDesc* d, u16* hufOut, u32* fseOut) {
     DecDesc L{};         // built in registers/local, stored by lane 0 at the end; mode 0: the fused kernel decodes the item
     L.outMax = 0xFFFFFFFFu;
     FrameHeader fh; u64 ref; u32 xxh;
-    if (frame_walk(src, srcSize, &fh, 1, &ref, &xxh) && !fh.checksum && fh.hasContentSize && fh.contentSize <= BLOCKSIZE_MAX) {
+    if (frame_walk(src, srcSize, &fh, 1, &ref, &xxh) && fh.hasContentSize && fh.contentSize <= BLOCKSIZE_MAX) {
         L.contentSize = (u32)fh.contentSize;
         if (w.lane == 0) { S.litEntropy = 0; S.fseEntropy = 0; }      // no earlier block: a repeated table is an error
         w.sync();
@@ -423,6 +462,7 @@ struct ExecShared {
     u32 tile[32];                // a round's bytes as far as they are known ...
     u32 late[32];                // ... which of them are not yet (bit t of word l: byte t of lane l) ...
     u32 link[32];                // ... and, for those, the byte of the round they copy (index inside the round, one byte each)
+    u32 sum[2];                  // the frame's checksum: whether it has one, the stored 32 bits (dec_exec)
 };
 // Index (relative to `cur`) of the sequence that holds output position p: the last of st[cur .. cur+63] that is <= p.  A round of
 // 128 bytes holds at most 43 sequence starts and st[cur] <= p for every byte that is looked up, so six halving steps decide.
@@ -447,8 +487,15 @@ ZB_HD u32 exec_mod(u32 a, u32 b) {
 #endif
 }
 
+// The n bytes at dst a checksummed frame regenerated (written by the whole warp, which has synchronised since) against the stored 32 bits
+// `want`: n, or checksum_wrong.  Not inlined: the hash's registers stay out of the executor's loop.
 template <class C>
-ZB_HD size_t dec_exec(const C& w, ExecShared& X, const DecDesc* dp, const u8* item, const u8* litBuf, const u64* seqs, u8* dst, size_t cap) {
+ZB_HDN size_t dec_checksum(const C& w, u32 want, const u8* dst, u32 n) {
+    return (u32)xxh64_warp(w, dst, n) == want ? n : ERR(E_checksum_wrong);
+}
+
+template <class C>
+ZB_HD size_t dec_exec_body(const C& w, ExecShared& X, const DecDesc* dp, const u8* item, const u8* litBuf, const u64* seqs, u8* dst, size_t cap) {
     DecDesc const& d = *dp;
     if (d.mode == 2 || d.mode == 3) {            // raw / rle block: 16-byte stores once dst is aligned
         u32 const n = d.mode == 2 ? d.cSize : d.regen;
@@ -662,6 +709,16 @@ ZB_HD size_t dec_exec(const C& w, ExecShared& X, const DecDesc* dp, const u8* it
         op += last;
         w.sync(); }
     return op == d.contentSize ? op : ERR(E_corruption_detected);
+}
+// Stage D, then the frame's checksum when it has one (the flag in its descriptor byte, the stored 32 bits right after its one block): the
+// fused decoder's checks in its order -- content size (corruption_detected), then checksum_wrong.
+// The two go through shared memory (X.sum), so that nothing of the item stays live in registers across stage D.
+template <class C>
+ZB_HD size_t dec_exec(const C& w, ExecShared& X, const DecDesc* dp, const u8* item, const u8* litBuf, const u64* seqs, u8* dst, size_t cap) {
+    if (w.lane == 0) { u32 const has = (item[4] >> 2) & 1; X.sum[0] = has; X.sum[1] = has ? load32(item + dp->blockOff + dp->cSize) : 0u; }
+    size_t const r = dec_exec_body(w, X, dp, item, litBuf, seqs, dst, cap);      // (a size comes back only after a warp synchronisation)
+    if (isErr(r) || !X.sum[0]) return r;
+    return dec_checksum(w, X.sum[1], dst, (u32)r);
 }
 
 }  // namespace zb
