@@ -186,16 +186,18 @@ ZSTDB200_API int zstdb200_device_count(void);
  * ZSTDB200_L2_FETCH (l2_fetch_granularity), ZSTDB200_HOST_SLICES, ZSTDB200_ENTROPY_OVERLAP and ZSTDB200_KERNEL_FIFO. */
 ZSTDB200_API int zstdb200_set_option(zstdb200_ctx* ctx, const char* name, long long value);
 ZSTDB200_API unsigned long long zstdb200_kernel_launches(const zstdb200_ctx* ctx);   /* kernels launched so far */
-/* frames of many blocks that zstdb200_decompress_batch gave to the segment decoder: regenerated there (deferred = 0), or handed to
+/* frames of many blocks that the host-memory decompression calls (zstdb200_decompress_batch, zstdb200_decompress_frames and
+ * zstdb200_decompress_frames_begin/_end) gave to the segment decoder: regenerated there (deferred = 0), or handed to
  * the fused kernel because the segment decoder could not vouch for them (deferred = 1: corrupted, short of capacity, wrong checksum)
  * or because the item of several frames they belong to was decoded again whole (see zstdb200_split_items) */
 ZSTDB200_API unsigned long long zstdb200_segment_frames(const zstdb200_ctx* ctx, int deferred);
-/* items of several frames that zstdb200_decompress_batch decoded frame by frame (deferred = 0: each frame as its own entry, on the
+/* items of several frames that the host-memory decompression calls decoded frame by frame (deferred = 0: each frame as its own entry, on the
  * staged, segment or fused decoder), or decoded again whole on the fused kernel because a frame did not regenerate exactly its
  * declared size or its checksum failed (deferred = 1).  An item is split when it is a whole number of frames (skippable ones included,
  * at least two), every zstd frame but the last declares its content size, those sizes fit the item's capacity, and its frames regenerate
  * at least 32 KB each on average; and only when the device workspaces of every frame (about 0.5 MB each) can be had -- otherwise the call
- * decodes every item whole, as with dec_pipeline 0.  With dec_pipeline 0 or on a magicless context no item is split. */
+ * decodes every item whole, as with dec_pipeline 0.  With dec_pipeline 0 no item is split.  On a magicless context the items are
+ * magicless frames (ZSTD_f_zstd1_magicless): they have no skippable frames, and are split and decoded by the same rules. */
 ZSTDB200_API unsigned long long zstdb200_split_items(const zstdb200_ctx* ctx, int deferred);
 
 /* Frame stream: one frame of many blocks decoded segment by segment as its blocks arrive, in memory that does not depend on the

@@ -19,7 +19,7 @@
 // An item is eligible when it is exactly one frame with one (last) block and carries its content size; a checksum is
 // verified at the end of stage D by the warp (xxh64_warp).  Everything else (multi-block, skippable, > MAXS sequences,
 // 2^12-cell Huffman tables) is left to the fused kernel or the segment decoder; an item of several frames is cut into
-// its frames first (item_walk, zstdb200_decompress_batch).  Results -- including the error code of corrupted input --
+// its frames first (item_walk, the decode list of the host-memory calls).  Results -- including the error code of corrupted input --
 // are identical to the fused path: the stage statuses are combined in the order the fused decoder would have met the errors.
 //
 // Reference behaviour reproduced: see zb_decode.cuh (N/decompress/zstd_decompress_block.c:134-340,695-775,
@@ -74,14 +74,14 @@ static_assert(sizeof(DecDesc) == 184 && offsetof(DecDesc, sBits) == 124 && offse
               offsetof(DecDesc, fseLog) == 156 && offsetof(DecDesc, hufLitSize) == 172 && offsetof(DecDesc, seqUnusable) == 176, "DecDesc layout");
 
 // ---------------------------------------------------------------------------------------- stage A
-// The blocks of an item that is exactly one frame of at most maxBlocks blocks: magic number, no dictionary, every block inside the item,
-// the checksum (when the frame has one) its last four bytes.  Returns the number of blocks (0: the item is not such a frame);
-// refs[k] = offset of block k's header | that header << 32 (refs may be null), *xxh = the stored checksum.
+// The blocks of an item that is exactly one frame of at most maxBlocks blocks: magic number (none when magicless), no dictionary, every
+// block inside the item, the checksum (when the frame has one) its last four bytes.  Returns the number of blocks (0: the item is not
+// such a frame); refs[k] = offset of block k's header | that header << 32 (refs may be null), *xxh = the stored checksum.
 // With `end`, the frame only has to start the item: *end = its size (frames past 4 GiB are not taken).
-ZB_HDN u32 frame_walk(const u8* src, size_t size, FrameHeader* fh, u32 maxBlocks, u64* refs, u32* xxh, size_t* end = nullptr) {
+ZB_HDN u32 frame_walk(const u8* src, size_t size, FrameHeader* fh, u32 maxBlocks, u64* refs, u32* xxh, size_t* end = nullptr, u32 magicless = 0) {
     if (end && size > 0xFFFFFFFFu) size = 0xFFFFFFFFu;
-    if (size < 9 || size > 0xFFFFFFFFu || load32(src) != MAGIC) return 0;
-    if (read_frame_header(fh, src, size) != 0 || fh->skippable || fh->dictID) return 0;
+    if (size < (magicless ? 5u : 9u) || size > 0xFFFFFFFFu || (!magicless && load32(src) != MAGIC)) return 0;
+    if (read_frame_header(fh, src, size, magicless) != 0 || fh->skippable || fh->dictID) return 0;
     size_t pos = fh->headerSize; u32 n = 0;
     for (;;) {
         if (size - pos < 3 || n == maxBlocks) return 0;
@@ -107,19 +107,21 @@ struct ItemFrame { u64 srcOff, srcSize, contentSize; u32 nBlocks, checksum, hasC
 // the walk stops where no whole frame follows.  *split: the item may be decoded frame by frame -- the walk covers it exactly, it has at
 // least two frames (skippable ones count), every zstd frame but the last declares its content size, and the declared sizes add up to
 // at most `capacity` (the last zstd frame, if it declares none, gets the rest).  Any other item is decoded whole.
-ZB_HDN u32 item_walk(const u8* src, size_t size, u64 capacity, ItemFrame* out, u32 outMax, bool* split) {
+// A magicless item has no skippable frames: bytes that read like a skippable magic number start a frame there, as in the reference
+// (N/decompress/zstd_decompress.c:744,1120).
+ZB_HDN u32 item_walk(const u8* src, size_t size, u64 capacity, ItemFrame* out, u32 outMax, bool* split, u32 magicless = 0) {
     u32 n = 0; size_t pos = 0; u64 declared = 0;
     bool sized = true, ok = true;      // sized: every zstd frame so far declares its content size
     while (pos < size) {
         ItemFrame f{}; FrameHeader fh;
         f.srcOff = pos;
         size_t const rest = size - pos;
-        if (rest >= 8 && (load32(src + pos) & 0xFFFFFFF0u) == 0x184D2A50u) {
+        if (!magicless && rest >= 8 && (load32(src + pos) & 0xFFFFFFF0u) == 0x184D2A50u) {
             if (read_frame_header(&fh, src + pos, rest) != 0 || (u64)fh.skipLen + 8 > rest) break;
             f.srcSize = 8 + (u64)fh.skipLen; f.skippable = 1;
         } else {
             size_t end = 0; u32 xxh;
-            u32 const nb = frame_walk(src + pos, rest, &fh, 0xFFFFFFFFu, nullptr, &xxh, &end);
+            u32 const nb = frame_walk(src + pos, rest, &fh, 0xFFFFFFFFu, nullptr, &xxh, &end, magicless);
             if (!nb) break;
             if (!sized) ok = false;                  // a zstd frame after one without a content size
             f.srcSize = end; f.nBlocks = nb; f.checksum = fh.checksum; f.hasContentSize = fh.hasContentSize; f.contentSize = fh.contentSize;
@@ -192,12 +194,14 @@ ZB_HD bool prepare_block(const C& w, DecShared& S, const u8* item, u32 off, u32 
 
 // The staged decoder takes an item that is one frame of one block, with its content size (at most one block); dec_exec verifies the
 // checksum when the frame has one.  All lanes of a warp; S is the warp's shared scratch; tables are copied out to hufOut / fseOut.
+// magicless: the item is in the ZSTD_f_zstd1_magicless format.
 template <class C>
-ZB_HDN void dec_prepare(const C& w, DecShared& S, const u8* src, size_t srcSize, size_t dstCapacity, DecDesc* d, u16* hufOut, u32* fseOut) {
+ZB_HDN void dec_prepare(const C& w, DecShared& S, const u8* src, size_t srcSize, size_t dstCapacity, DecDesc* d, u16* hufOut, u32* fseOut,
+                        u32 magicless = 0) {
     DecDesc L{};         // built in registers/local, stored by lane 0 at the end; mode 0: the fused kernel decodes the item
     L.outMax = 0xFFFFFFFFu;
     FrameHeader fh; u64 ref; u32 xxh;
-    if (frame_walk(src, srcSize, &fh, 1, &ref, &xxh) && fh.hasContentSize && fh.contentSize <= BLOCKSIZE_MAX) {
+    if (frame_walk(src, srcSize, &fh, 1, &ref, &xxh, nullptr, magicless) && fh.hasContentSize && fh.contentSize <= BLOCKSIZE_MAX) {
         L.contentSize = (u32)fh.contentSize;
         if (w.lane == 0) { S.litEntropy = 0; S.fseEntropy = 0; }      // no earlier block: a repeated table is an error
         w.sync();
@@ -710,12 +714,13 @@ ZB_HD size_t dec_exec_body(const C& w, ExecShared& X, const DecDesc* dp, const u
         w.sync(); }
     return op == d.contentSize ? op : ERR(E_corruption_detected);
 }
-// Stage D, then the frame's checksum when it has one (the flag in its descriptor byte, the stored 32 bits right after its one block): the
-// fused decoder's checks in its order -- content size (corruption_detected), then checksum_wrong.
-// The two go through shared memory (X.sum), so that nothing of the item stays live in registers across stage D.
+// Stage D, then the frame's checksum when it has one (the flag in its descriptor byte, after the magic number unless magicless; the
+// stored 32 bits right after its one block): the fused decoder's checks in its order -- content size (corruption_detected), then
+// checksum_wrong.  The two go through shared memory (X.sum), so that nothing of the item stays live in registers across stage D.
 template <class C>
-ZB_HD size_t dec_exec(const C& w, ExecShared& X, const DecDesc* dp, const u8* item, const u8* litBuf, const u64* seqs, u8* dst, size_t cap) {
-    if (w.lane == 0) { u32 const has = (item[4] >> 2) & 1; X.sum[0] = has; X.sum[1] = has ? load32(item + dp->blockOff + dp->cSize) : 0u; }
+ZB_HD size_t dec_exec(const C& w, ExecShared& X, const DecDesc* dp, const u8* item, const u8* litBuf, const u64* seqs, u8* dst, size_t cap,
+                      u32 magicless = 0) {
+    if (w.lane == 0) { u32 const has = (item[magicless ? 0 : 4] >> 2) & 1; X.sum[0] = has; X.sum[1] = has ? load32(item + dp->blockOff + dp->cSize) : 0u; }
     size_t const r = dec_exec_body(w, X, dp, item, litBuf, seqs, dst, cap);      // (a size comes back only after a warp synchronisation)
     if (isErr(r) || !X.sum[0]) return r;
     return dec_checksum(w, X.sum[1], dst, (u32)r);

@@ -1,4 +1,4 @@
-// zb_decode_list.cuh -- host side of zstdb200_decompress_batch: the decode list, which cuts items of several frames into their frames.
+// zb_decode_list.cuh -- host side of the host-memory decompression calls: the decode list, which cuts items of several frames into their frames.
 //
 // An item item_walk lets split (zb_decode_fast.cuh) becomes one entry per frame -- a skippable frame too: it regenerates nothing, so
 // its capacity is 0 -- output at the item's output plus the declared sizes of the frames before it, capacity its own declared size (the
@@ -25,12 +25,16 @@ struct DecodeList {
     std::vector<u64> src, dst;           // entry j: input [src[j], src[j + 1]), output [dst[j], dst[j + 1]) (m + 1 each)
     std::vector<size_t> first;           // item i: entries [first[i], first[i + 1])
     std::vector<ItemFrame> frame;        // the frame of each entry of a split item (unused for the others)
+    std::vector<ItemFrame> walked;       // planning scratch: the frames of the items to split, in item order
+    std::vector<u32> count;              // ... and how many each has
 };
 
 // n items back to back at `staged`: item i's input [srcOff[i], srcOff[i + 1]), its output [dstOff[i], dstOff[i + 1]) (both n + 1 long).
-// pipeline false: every item whole.  reserve(m) -> whether the workspaces of m entries could be had.
+// pipeline false: every item whole.  reserve(m) -> whether the workspaces of m entries could be had.  magicless: the items are in the
+// ZSTD_f_zstd1_magicless format.  The list's vectors keep their storage from one plan to the next.
 template <class Reserve>
-void plan_decode_list(DecodeList& L, size_t n, const u8* staged, const u64* srcOff, const u64* dstOff, bool pipeline, Reserve reserve) {
+void plan_decode_list(DecodeList& L, size_t n, const u8* staged, const u64* srcOff, const u64* dstOff, bool pipeline, Reserve reserve,
+                      u32 magicless = 0) {
     auto whole = [&] {
         L.m = n; L.split.assign(n, 0); L.frame.clear();
         L.src.assign(srcOff, srcOff + n + 1); L.dst.assign(dstOff, dstOff + n + 1);
@@ -39,18 +43,19 @@ void plan_decode_list(DecodeList& L, size_t n, const u8* staged, const u64* srcO
     whole();
     if (!pipeline) return;
     try {
-        std::vector<ItemFrame> frames;      // the frames of the items to split, in item order
-        std::vector<u32> count(n, 0);       // ... and how many each has
+        std::vector<ItemFrame>& frames = L.walked;
+        std::vector<u32>& count = L.count;
+        frames.clear(); count.assign(n, 0);
         size_t m = n;
         for (size_t i = 0; i < n; i++) {
             size_t const size = (size_t)(srcOff[i + 1] - srcOff[i]);
             u64 const cap = dstOff[i + 1] - dstOff[i];
             bool ok = false;
-            u32 const nf = item_walk(staged + srcOff[i], size, cap, nullptr, 0, &ok);
+            u32 const nf = item_walk(staged + srcOff[i], size, cap, nullptr, 0, &ok, magicless);
             if (!ok) continue;
             size_t const at = frames.size();
             frames.resize(at + nf);
-            item_walk(staged + srcOff[i], size, cap, frames.data() + at, nf, &ok);
+            item_walk(staged + srcOff[i], size, cap, frames.data() + at, nf, &ok, magicless);
             u64 bytes = 0;      // what the item's frames regenerate: their declared sizes, or all of the capacity when the last declares none
             for (size_t k = at; k < at + nf; k++) if (!frames[k].skippable) bytes = frames[k].hasContentSize ? bytes + frames[k].contentSize : cap;
             if (bytes / nf < SPLIT_MIN_BYTES) { frames.resize(at); continue; }
@@ -58,22 +63,21 @@ void plan_decode_list(DecodeList& L, size_t n, const u8* staged, const u64* srcO
         }
         if (m == n) return;
         if (m > 0x7FFFFFFFull || !reserve(m)) { whole(); return; }
-        std::vector<u64> src, dst; std::vector<size_t> first(n + 1); std::vector<ItemFrame> frame(m);
-        src.reserve(m + 1); dst.reserve(m + 1);
+        L.src.clear(); L.dst.clear(); L.frame.resize(m);
         size_t k = 0;
         for (size_t i = 0; i < n; i++) {
-            first[i] = src.size();
-            if (!L.split[i]) { src.push_back(srcOff[i]); dst.push_back(dstOff[i]); continue; }
+            L.first[i] = L.src.size();
+            if (!L.split[i]) { L.src.push_back(srcOff[i]); L.dst.push_back(dstOff[i]); continue; }
             u64 d = dstOff[i];
             for (u32 q = 0; q < count[i]; q++) {
                 ItemFrame const& f = frames[k++];
-                frame[src.size()] = f;
-                src.push_back(srcOff[i] + f.srcOff); dst.push_back(d);
+                L.frame[L.src.size()] = f;
+                L.src.push_back(srcOff[i] + f.srcOff); L.dst.push_back(d);
                 if (!f.skippable) d += f.hasContentSize ? f.contentSize : dstOff[i + 1] - d;
             }
         }
-        src.push_back(srcOff[n]); dst.push_back(dstOff[n]); first[n] = m;
-        L.m = m; L.src.swap(src); L.dst.swap(dst); L.first.swap(first); L.frame.swap(frame);
+        L.src.push_back(srcOff[n]); L.dst.push_back(dstOff[n]); L.first[n] = m;
+        L.m = m;
     } catch (const std::bad_alloc&) {
         whole();
     }

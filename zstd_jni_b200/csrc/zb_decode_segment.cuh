@@ -83,10 +83,10 @@ struct SegCarry {
 // The largest window the segment decoder takes (the default windowLogMax): larger ones stay with the fused decoder.
 constexpr u64 SEG_WINDOW_MAX = 1ull << 27;
 
-// Host side: the blocks of an item the segment decoder takes, one frame (frame_walk) of more than one block with a window of at most
-// SEG_WINDOW_MAX.  Returns the number of blocks, 0 for any other item.
-ZB_HDN u32 seg_walk(const u8* src, size_t size, FrameHeader* fh, u64* refs, u32* xxh) {
-    u32 const n = frame_walk(src, size, fh, 0xFFFFFFFFu, refs, xxh);
+// Host side: the blocks of an item the segment decoder takes, one frame (frame_walk, in the format `magicless` names) of more than one
+// block with a window of at most SEG_WINDOW_MAX.  Returns the number of blocks, 0 for any other item.
+ZB_HDN u32 seg_walk(const u8* src, size_t size, FrameHeader* fh, u64* refs, u32* xxh, u32 magicless = 0) {
+    u32 const n = frame_walk(src, size, fh, 0xFFFFFFFFu, refs, xxh, nullptr, magicless);
     return n >= 2 && fh->windowSize <= SEG_WINDOW_MAX ? n : 0;
 }
 
