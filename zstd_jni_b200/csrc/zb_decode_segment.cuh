@@ -64,15 +64,19 @@ struct SegBlock {
     u32 hufSrc, fseSrc[3];    // segment block whose table the block uses, or SEG_CARRY
     u32 bad;             // the frame goes to the fused decoder
     u32 regen;
-    u64 out;             // frame position of the block's first output byte
+    u64 out;             // item position of the block's first output byte (a frame of its own: frame position)
+    u64 frameAt, segAt;  // item positions of its frame's first output byte and of its item's first output byte in the segment
+    u32 linkAt;          // link map entry of the byte at segAt
     u64 sumLL, sumML;
     u32 rep[3];          // repcode history at the block's start
     RepSym sum[3];       // ... and at its end, as functions of rep
 };
 
 struct SegCarry {
-    u64 pos, cap;        // output bytes of the frame so far, output capacity of the item
+    u64 pos, cap;        // output bytes of the item so far, output capacity of the item
+    u64 frameAt;         // item position where the frame in progress starts
     u32 bad;
+    u32 links;           // link map entries of the segment just scanned
     u32 hasHuf, hufLog, hasFse, fseLog[3];
     u32 rep[3];
     u32 nextHuf, nextFse[3];  // the last describing blocks of the segment just prepared (SEG_CARRY / SEG_NONE: none there)
@@ -88,6 +92,105 @@ constexpr u64 SEG_WINDOW_MAX = 1ull << 27;
 ZB_HDN u32 seg_walk(const u8* src, size_t size, FrameHeader* fh, u64* refs, u32* xxh, u32 magicless = 0) {
     u32 const n = frame_walk(src, size, fh, 0xFFFFFFFFu, refs, xxh, nullptr, magicless);
     return n >= 2 && fh->windowSize <= SEG_WINDOW_MAX ? n : 0;
+}
+
+// ---------------------------------------------------------------------------------------- the device call's loop
+// zstdb200_decompress_device plans on the GPU: each item is walked there (seg_item_blocks), and the blocks of all the items the loop takes
+// form one sequence, cut into segments of B blocks that may cross frame and item boundaries.  A block carries its place in it (SegLoc);
+// at a frame start the stages drop the earlier tables and restart the repcodes, at an item start the output position.  Any doubt marks
+// the whole item in `itemBad`, and the fused decoder decodes it again; the loop decides no error.
+
+// The blocks of an item the loop takes: a whole number of frames -- zstd frames (frame_walk) with a window of at most SEG_WINDOW_MAX,
+// skippable ones unless magicless -- at least one zstd frame, and a frame of two blocks or two frames.  0 for any other item.
+ZB_HDN u64 seg_item_blocks(const u8* src, size_t size, u32 magicless) {
+    if (size > 0xFFFFFFFFu) return 0;
+    size_t pos = 0; u64 blocks = 0; u32 frames = 0, zframes = 0, most = 0;
+    while (pos < size) {
+        size_t const rest = size - pos;
+        if (!magicless && rest >= 8 && (load32(src + pos) & 0xFFFFFFF0u) == 0x184D2A50u) {
+            if ((u64)load32(src + pos + 4) + 8 > rest) return 0;
+            pos += 8 + (size_t)load32(src + pos + 4);
+        } else {
+            FrameHeader fh; size_t end = 0; u32 xxh;
+            u32 const nb = frame_walk(src + pos, rest, &fh, 0xFFFFFFFFu, nullptr, &xxh, &end, magicless);
+            if (!nb || fh.windowSize > SEG_WINDOW_MAX) return 0;
+            blocks += nb; zframes++; most = nb > most ? nb : most; pos += end;
+        }
+        frames++;
+    }
+    return zframes && (most >= 2 || frames >= 2) ? blocks : 0;
+}
+
+// A block of the loop: its item, its frame's blockSizeMax, and flags -- it starts its item, starts its frame, ends its frame (then with
+// the frame's stored checksum and declared content size when it has them); cap: the item's output capacity.
+struct SegLoc { u32 item, flags, blockSizeMax, xxh; u64 cap, contentSize; };
+constexpr u32 LOC_ITEM = 1, LOC_FRAME = 2, LOC_END = 4, LOC_CHECKSUM = 8, LOC_SIZE = 16;
+
+// Which candidates go to the loop.  The loop decodes its blocks one segment after another, at about the same rate whatever their items;
+// the fused kernel decodes `warps` items at once, each with one warp that is about SEG_FUSED_BLOCK_COST times slower per block than the
+// loop (H100, level-3 frames: 0.011 GB/s per warp against 2.1 GB/s for the loop).  So a few long items belong on the loop and many short
+// ones on the fused kernel.  The candidates are counted in buckets of floor(log2(blocks)) -- cnt, sum and max of the block counts -- and
+// the least number of blocks an item needs to go to the loop is the power of two with the least estimated time of the fused kernel
+// (the longer of its longest item and its blocks spread over the warps) plus the loop (its blocks); ~0 sends every item to the fused kernel.
+constexpr u32 SEG_BUCKETS = 33;
+constexpr u64 SEG_FUSED_BLOCK_COST = 200;
+ZB_HDN u64 seg_loop_min_blocks(const u32* cnt, const u64* sum, const u32* max, u64 warps) {
+    u64 loop = 0;
+    for (u32 k = 0; k < SEG_BUCKETS; k++) loop += sum[k];
+    u64 best = ~0ull, bestCost = ~0ull, fusedSum = 0, fusedMax = 0;
+    for (u32 k = 0; k <= SEG_BUCKETS; k++) {      // items of fewer than 2^k blocks fused, the others on the loop
+        u64 const spread = (fusedSum + warps - 1) / warps, fused = (fusedMax > spread ? fusedMax : spread) * SEG_FUSED_BLOCK_COST;
+        if (fused + loop < bestCost) { bestCost = fused + loop; best = k < SEG_BUCKETS ? 1ull << k : ~0ull; }
+        if (k < SEG_BUCKETS) { fusedSum += sum[k]; loop -= sum[k]; if (cnt[k] && max[k] > fusedMax) fusedMax = max[k]; }
+    }
+    return best;
+}
+// The bucket of an item of b >= 1 blocks.
+ZB_HD u32 seg_bucket(u64 b) { u32 k = 0; while (k + 1 < SEG_BUCKETS && (b >> (k + 1))) k++; return k; }
+
+// The loop's cursor: the call's items (list[0 .. count): the loop's, in the order walked) and the walk's position among their blocks.
+struct SegCursor {
+    const u8* src; const u64* srcOff; u8* dst; const u64* dstOff; u64* results;
+    u32* itemBad;                // per item of the call: nonzero when the fused decoder decodes it again
+    u32* list; u32 count, magicless;
+    u32 k, at, inFrame, first;   // list index, byte offset in its item, 1 inside a frame (2: before its first block), next block starts the item
+    u32 blockSizeMax, checksum, hasSize; u64 contentSize;      // the frame walked
+    u32 n;                       // blocks in the segment walked last
+    u32 cnt[SEG_BUCKETS], max[SEG_BUCKETS]; u64 sum[SEG_BUCKETS];      // the candidates (seg_loop_min_blocks)
+    u64 minBlocks;               // the least blocks of an item on the loop
+};
+
+// Walks the next segment: up to B blocks from the cursor into refs (offset in the item | header << 32) and loc; returns their number.
+// The items were walked whole before (seg_item_blocks), so every header read here is inside its item.
+ZB_HDN u32 seg_walk_segment(SegCursor* c, u32 B, u64* refs, SegLoc* loc) {
+    u32 n = 0;
+    while (n < B && c->k < c->count) {
+        u32 const item = c->list[c->k];
+        const u8* const src = c->src + c->srcOff[item];
+        u32 const size = (u32)(c->srcOff[item + 1] - c->srcOff[item]);
+        if (!c->inFrame) {
+            if (c->at == size) { c->k++; c->at = 0; c->first = 1; continue; }
+            if (!c->magicless && size - c->at >= 8 && (load32(src + c->at) & 0xFFFFFFF0u) == 0x184D2A50u) { c->at += 8 + load32(src + c->at + 4); continue; }
+            FrameHeader fh;
+            read_frame_header(&fh, src + c->at, size - c->at, c->magicless);
+            c->blockSizeMax = fh.blockSizeMax; c->checksum = fh.checksum; c->hasSize = fh.hasContentSize; c->contentSize = fh.contentSize;
+            c->at += fh.headerSize; c->inFrame = 2;
+        }
+        u32 const bh = load24(src + c->at), cSize = ((bh >> 1) & 3) == 1 ? 1 : bh >> 3;
+        SegLoc L;
+        L.item = item; L.blockSizeMax = c->blockSizeMax; L.xxh = 0; L.cap = c->dstOff[item + 1] - c->dstOff[item]; L.contentSize = c->contentSize;
+        L.flags = (c->first ? LOC_ITEM : 0u) | (c->inFrame == 2 ? LOC_FRAME : 0u);
+        refs[n] = (u64)c->at | ((u64)bh << 32);
+        c->at += 3 + cSize; c->first = 0; c->inFrame = 1;
+        if (bh & 1) {
+            L.flags |= LOC_END | (c->checksum ? LOC_CHECKSUM : 0u) | (c->hasSize ? LOC_SIZE : 0u);
+            if (c->checksum) { L.xxh = load32(src + c->at); c->at += 4; }
+            c->inFrame = 0;
+        }
+        loc[n++] = L;
+    }
+    c->n = n;
+    return n;
 }
 
 // ---------------------------------------------------------------------------------------- stage A
@@ -114,25 +217,32 @@ ZB_HDN void seg_prepare(const C& w, DecShared& S, const u8* frame, u32 off, u32 
 // ---------------------------------------------------------------------------------------- stage B
 // In block order: the table every repeating block reuses (ZSTD_decodeLiteralsBlock :148 / ZSTD_buildSeqTable :686).  The first
 // segment of a frame starts the carried state.
-ZB_HDN void seg_tables(SegBlock* blocks, u32 n, SegCarry* c, bool first, u64 cap) {
+// In the loop (loc, itemBad): at a frame start no earlier table; a failing block marks its item and the walk goes on with the next one.
+ZB_HDN void seg_tables(SegBlock* blocks, u32 n, SegCarry* c, bool first, u64 cap, const SegLoc* loc = nullptr, u32* itemBad = nullptr) {
     if (first) {
-        c->pos = 0; c->cap = cap; c->bad = 0; c->hasHuf = 0; c->hasFse = 0;
+        c->pos = 0; c->cap = cap; c->bad = 0; c->hasHuf = 0; c->hasFse = 0; c->frameAt = 0;
         c->rep[0] = 1; c->rep[1] = 4; c->rep[2] = 8;
     }
     u32 huf = c->hasHuf ? SEG_CARRY : SEG_NONE, fse[3];
     for (int t = 0; t < 3; t++) fse[t] = c->hasFse ? SEG_CARRY : SEG_NONE;
     for (u32 j = 0; j < n && !c->bad; j++) {
         SegBlock& B = blocks[j];
-        if (B.bad) { c->bad = 1; break; }
+        u32* const bad = loc ? itemBad + loc[j].item : &c->bad;
+        if (loc && (loc[j].flags & LOC_FRAME)) {
+            huf = SEG_NONE; c->hasHuf = 0; c->hasFse = 0;
+            for (int t = 0; t < 3; t++) fse[t] = SEG_NONE;
+        }
+        if (*bad) continue;
+        if (B.bad) { *bad = 1; continue; }
         if (B.d.mode != 1) continue;
         if (B.litType == 3) {
-            if (huf == SEG_NONE) { c->bad = 1; break; }
+            if (huf == SEG_NONE) { *bad = 1; continue; }
             B.hufSrc = huf; B.d.hufLog = huf == SEG_CARRY ? c->hufLog : blocks[huf].d.hufLog;
         } else if (B.litType == 2) huf = j;
         if (B.d.nbSeq) {
             for (int t = 0; t < 3; t++) {
                 if ((B.fseRepeat >> t) & 1) {
-                    if (fse[t] == SEG_NONE) { c->bad = 1; break; }
+                    if (fse[t] == SEG_NONE) { *bad = 1; break; }
                     B.d.fseLog[t] = fse[t] == SEG_CARRY ? c->fseLog[t] : blocks[fse[t]].d.fseLog[t];
                 } else fse[t] = j;
                 B.fseSrc[t] = fse[t];
@@ -179,20 +289,31 @@ ZB_HDN void seg_seq(SegBlock* blocks, u32 j, const u8* frame, const u32* fseBase
     B.sumLL = sLL; B.sumML = sML;
 }
 
-// Output positions and start histories, in block order (after stage C); `last`: the frame's final segment.
-ZB_HDN void seg_scan(SegBlock* blocks, u32 n, SegCarry* c, u32 blockSizeMax) {
+// Output positions and start histories, in block order (after stage C).  Every block gets its item position (out), its frame's (frameAt)
+// and its place in the link map: the item's bytes of the segment from segAt on are the entries from linkAt on.  In the loop a block
+// starting an item starts its position at 0 and its capacity at loc's, a block starting a frame restarts the repcodes there.
+ZB_HDN void seg_scan(SegBlock* blocks, u32 n, SegCarry* c, u32 blockSizeMax, const SegLoc* loc = nullptr, u32* itemBad = nullptr) {
     if (c->bad) return;
-    u64 pos = c->pos;
-    u32 rep[3] = { c->rep[0], c->rep[1], c->rep[2] };
+    u64 pos = c->pos, cap = c->cap, frameAt = c->frameAt, segAt = pos;
+    u32 rep[3] = { c->rep[0], c->rep[1], c->rep[2] }, links = 0, linkAt = 0;
     for (u32 j = 0; j < n; j++) {
         SegBlock& B = blocks[j];
+        u32* bad = &c->bad; u32 bsm = blockSizeMax;
+        if (loc) {
+            SegLoc const& L = loc[j];
+            bad = itemBad + L.item; bsm = L.blockSizeMax;
+            if (L.flags & LOC_ITEM) { pos = 0; cap = L.cap; segAt = 0; linkAt = links; }
+            if (L.flags & LOC_FRAME) { frameAt = pos; rep[0] = 1; rep[1] = 4; rep[2] = 8; }
+        }
+        B.out = pos; B.frameAt = frameAt; B.segAt = segAt; B.linkAt = linkAt; B.regen = 0;
+        if (*bad) continue;
         u64 regen = B.d.regen;
         if (B.d.mode == 1) {
-            if (B.bad || B.d.stB || B.d.stC || B.sumLL > B.d.litSize) { c->bad = 1; return; }
+            if (B.bad || B.d.stB || B.d.stC || B.sumLL > B.d.litSize) { *bad = 1; if (loc) continue; return; }
             regen = B.d.litSize + B.sumML;
         }
-        if (regen > blockSizeMax || regen > c->cap - pos) { c->bad = 1; return; }
-        B.regen = (u32)regen; B.out = pos; pos += regen;
+        if (regen > bsm || regen > cap - pos) { *bad = 1; if (loc) continue; return; }
+        B.regen = (u32)regen; pos += regen; links += (u32)regen;
         for (int s = 0; s < 3; s++) B.rep[s] = rep[s];
         if (B.d.mode == 1 && B.d.nbSeq) {
             u32 nr[3];
@@ -200,7 +321,7 @@ ZB_HDN void seg_scan(SegBlock* blocks, u32 n, SegCarry* c, u32 blockSizeMax) {
             for (int s = 0; s < 3; s++) rep[s] = nr[s];
         }
     }
-    c->pos = pos;
+    c->pos = pos; c->cap = cap; c->frameAt = frameAt; c->links = links;
     for (int s = 0; s < 3; s++) c->rep[s] = rep[s];
 }
 
@@ -231,17 +352,18 @@ ZB_HD void seg_carry_tables(const C& w, const SegBlock* blocks, const u16* hufBa
 }
 
 // ---------------------------------------------------------------------------------------- stage D
-// Block j's bytes into the link map of the segment that starts at frame position segStart: literal bytes and bytes copied from before
-// the segment are final, a match byte inside the segment names the byte it copies -- for a match that overlaps itself, the byte of its
+// Block j's bytes into the segment's link map (entry linkAt + p - segAt for item position p): literal bytes and bytes copied from before
+// the segment are final, a match byte inside the segment names the entry it copies -- for a match that overlaps itself, the byte of its
 // first period, so that a run is one link deep.  Sequences go 32 at a time, their bytes are spread over the lanes.
 struct SegRec { u64 o, md; u32 ls, off; };
-// `hist`: the output before the segment, frame position p at hist[p & mask]; an offset beyond `window` marks the frame bad.
+// `hist`: the item's output before the segment, item position p at hist[p & mask]; an offset before the frame or beyond `window` sets
+// *bad.
 template <class C>
 ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const u8* frame, const u8* lit, const u64* seqs, const u32* offs,
-                     const u8* hist, u64 mask, u64 window, u64 segStart, u32* link, SegCarry* c) {
+                     const u8* hist, u64 mask, u64 window, u32* link, u32* bad) {
     SegBlock const& B = blocks[j];
     u64 const base = B.out;
-    auto put = [&](u64 p, u32 v) { link[p - segStart] = v; };
+    auto put = [&](u64 p, u32 v) { link[B.linkAt + (p - B.segAt)] = v; };
     if (B.d.mode == 2 || B.d.mode == 3) {
         const u8* const s = frame + B.d.blockOff;
         for (u32 i = (u32)w.lane; i < B.regen; i += C::W) put(base + i, SEG_FINAL | (B.d.mode == 2 ? s[i] : B.d.rleByte));
@@ -257,8 +379,8 @@ ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const
         u32 const ll = (u32)(q & 0x3FFFF), ml = (u32)((q >> 18) & 0x3FFFF), off = i < B.d.nbSeq ? offs[i] : 0;
         u64 const o = op + w.exscan(ll + ml);
         u32 const ls = lp + w.exscan(ll);
-        bool const bad = i < B.d.nbSeq && ((u64)off > o + ll || off > window);     // before the frame (ZSTD_execSequence :1034) or the window
-        if (w.ballot(bad)) { if (w.lane == 0) c->bad = 1; return; }
+        bool const far = i < B.d.nbSeq && ((u64)off > o + ll - B.frameAt || off > window);     // before the frame (ZSTD_execSequence :1034) or the window
+        if (w.ballot(far)) { if (w.lane == 0) *bad = 1; return; }
         SegRec r; r.o = o; r.md = o + ll; r.ls = ls; r.off = off;
         R[w.lane] = r;
         u32 const cnt = B.d.nbSeq - s0 < (u32)C::W ? B.d.nbSeq - s0 : (u32)C::W;
@@ -273,7 +395,7 @@ ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const
             if (p < e.md) v = SEG_FINAL | (rle ? B.d.rleByte : L[e.ls + (u32)(p - e.o)]);
             else {
                 u64 const src = e.md - e.off + (p - e.md) % e.off;
-                v = src < segStart ? SEG_FINAL | hist[src & mask] : (u32)(src - segStart);
+                v = src < B.segAt ? SEG_FINAL | hist[src & mask] : B.linkAt + (u32)(src - B.segAt);
             }
             put(p, v);
         }
@@ -284,7 +406,14 @@ ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const
     w.sync();
 }
 
-// The history is the frame's whole output in dst.
+// One frame a segment at a time (segStart: blocks[0].out, which the blocks carry as segAt): the history at hist[p & mask], or the frame's
+// whole output in dst.
+template <class C>
+ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const u8* frame, const u8* lit, const u64* seqs, const u32* offs,
+                     const u8* hist, u64 mask, u64 window, u64 segStart, u32* link, SegCarry* c) {
+    (void)segStart;
+    seg_fill(w, R, blocks, j, frame, lit, seqs, offs, hist, mask, window, link, &c->bad);
+}
 template <class C>
 ZB_HDN void seg_fill(const C& w, SegRec* R, const SegBlock* blocks, u32 j, const u8* frame, const u8* lit, const u64* seqs, const u32* offs,
                      const u8* dst, u64 segStart, u32* link, SegCarry* c) {
@@ -299,6 +428,18 @@ ZB_HD u8 seg_jump(volatile u32* link, u32 p) {
     return (u8)v;
 }
 
+
+// The loop's frame that ends with block j (LOC_END), its item not marked: its declared content size, and its checksum over its output
+// dst[frameAt, end) with the whole warp.  Either wrong marks the item.  Returns the item position where the frame ends.
+template <class C>
+ZB_HDN u64 seg_frame_end(const C& w, const SegBlock* blocks, u32 j, const SegLoc& L, const u8* dst, u32* bad) {
+    SegBlock const& B = blocks[j];
+    u64 const end = B.out + B.regen, len = end - B.frameAt;
+    bool ok = !(L.flags & LOC_SIZE) || len == L.contentSize;
+    if (ok && (L.flags & LOC_CHECKSUM)) ok = (u32)xxh64_warp(w, dst + B.frameAt, (size_t)len) == L.xxh;
+    if (!ok && w.lane == 0) *bad = 1;
+    return end;
+}
 
 // ---------------------------------------------------------------------------------------- resume
 // The fused decoder (zb_decode.cuh) from a block boundary: the n blocks at in + (u32)refs[j] (headers refs[j] >> 32) of the segment that
@@ -371,7 +512,7 @@ ZB_HD size_t stream_resume_result(size_t r) { return r == ERR(E_dstSize_tooSmall
 
 // The carried state at the start of a frame, before its first segment (what seg_tables sets up for `first`).
 ZB_HD void seg_carry_init(SegCarry* c, u64 cap) {
-    c->pos = 0; c->cap = cap; c->bad = 0; c->hasHuf = 0; c->hasFse = 0; c->hufLog = 0;
+    c->pos = 0; c->cap = cap; c->frameAt = 0; c->bad = 0; c->hasHuf = 0; c->hasFse = 0; c->hufLog = 0;
     c->rep[0] = 1; c->rep[1] = 4; c->rep[2] = 8;
     for (int t = 0; t < 3; t++) c->fseLog[t] = 0;
 }
