@@ -312,12 +312,16 @@ ZSTDB200_API size_t zstdb200_compact_device(zstdb200_ctx* ctx, size_t n, const v
                                             void* d_out, uint64_t* d_outOffsets, void* stream);
 /* decompress_device regenerates item i into d_dst + d_dstOffsets[i] (capacity d_dstOffsets[i+1] - d_dstOffsets[i]) and writes its size or
  * error code to d_results[i].  With dec_pipeline on (the default) the items are routed on the GPU: single-block frames with a content size
- * go to the staged decoder; items that are a whole number of frames with a frame of several blocks or several frames (windows <= 2^27,
- * skippable frames allowed, content sizes optional) go to a segment loop that a CUDA graph drives on the GPU over the blocks of all of
- * them when they are long or few -- many short ones decode faster one warp each -- and everything else to the fused kernel, which also
- * decodes again whole every item the loop doubts; results are those of the fused
+ * go to the staged decoder; items of several frames that are all one block are cut into their frames on the GPU, by the rule the
+ * host-memory calls follow (every frame but the last declares its content size, at least 32 KB regenerated per frame on average), and
+ * a CUDA graph runs the staged decoder over those frames in parts of 512 to 16384 (n); other items that are a whole number of frames with
+ * a frame of several blocks or several frames (windows <= 2^27, skippable frames allowed, content sizes optional) go to a segment loop
+ * that a CUDA graph drives on the GPU over the blocks of all of them when they are long or few -- many short ones decode faster one
+ * warp each -- and everything else to the fused kernel, which also decodes again whole every item the loop doubts and every split item
+ * whose frames do not each regenerate their declared size; results are those of the fused
  * decoder.  Nothing in the call waits on the host.  The loop's workspace (about 1.2 MB per dec_segment_blocks block, 600 MB at the
  * default) is allocated on the context's first such call and kept; when it or the graph cannot be had the call routes without the loop.
+ * The split's list (about 52 bytes per entry, 2^16 + 16 n entries) is kept likewise; when it or its graph cannot be had no item is split.
  * The call uses the context's work set 0 and must not overlap another call on it.  zstdb200_segment_frames and zstdb200_split_items
  * do not count device calls. */
 ZSTDB200_API size_t zstdb200_decompress_device(zstdb200_ctx* ctx, size_t n, const void* d_src, const uint64_t* d_srcOffsets,

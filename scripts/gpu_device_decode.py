@@ -5,10 +5,12 @@ against the fused kernel alone (dec_pipeline 0).  Warm, best of 3, outputs compa
                        frame (host memory in and out) in the same session
   frame-L3-xxh:        the level-3 frame with a checksum: the device call, whose difference to frame-L3 is the cost of the device XXH64
   items-64x128K:       128 items of 64 concatenated 128 KB level-3 frames: the device call with dec_pipeline 1 and 0
+  singles-128K:        8192 items of one 128 KB level-3 frame: the device call
   files-256K:          8192 items of one 256 KB level-3 frame (two blocks, as the zstd tool writes such a file): the device call
   items-2to4x128K:     4096 items of 2-4 concatenated 128 KB level-3 frames: the device call
-The last two are many short items, which the device call leaves to the fused kernel; the first ones are few long items, which it
-decodes on the segment loop.  Prints one JSON line with the card's name and power limit.
+The one-frame items go to the staged decoder, the two-block files to the fused kernel (many short items), the long frames to the
+segment loop; the items of several one-block frames are cut into their frames for the staged decoder.  Prints one JSON line with the
+card's name and power limit.
     python scripts/gpu_device_decode.py [--mb 1024] [--lib path/to/libzstdb200.so] [--many-only]
 --lib measures another build of the library (an earlier commit); --many-only times only the many-item workloads (an earlier build
 decodes the long items with one warp each, minutes per GiB).
@@ -96,6 +98,7 @@ def main():
         res["files-256K"] = {"device": device_rate(ctx, [frames[i % 64] for i in range(8192)], [parts[i % 64] for i in range(8192)])}
         small = [text(chunk, 400 + k) for k in range(64)]
         sframes = [ref_compress_flags(p, 3) for p in small]
+        res["singles-128K"] = {"device": device_rate(ctx, [sframes[i % 64] for i in range(8192)], [small[i % 64] for i in range(8192)])}
         groups = [[(g * 7 + j) % 64 for j in range(2 + g % 3)] for g in range(64)]
         res["items-2to4x128K"] = {"device": device_rate(ctx, [b"".join(sframes[j] for j in groups[i % 64]) for i in range(4096)],
                                                         [b"".join(small[j] for j in groups[i % 64]) for i in range(4096)])}

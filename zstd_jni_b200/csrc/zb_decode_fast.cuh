@@ -109,7 +109,11 @@ struct ItemFrame { u64 srcOff, srcSize, contentSize; u32 nBlocks, checksum, hasC
 // at most `capacity` (the last zstd frame, if it declares none, gets the rest).  Any other item is decoded whole.
 // A magicless item has no skippable frames: bytes that read like a skippable magic number start a frame there, as in the reference
 // (N/decompress/zstd_decompress.c:744,1120).
-ZB_HDN u32 item_walk(const u8* src, size_t size, u64 capacity, ItemFrame* out, u32 outMax, bool* split, u32 magicless = 0) {
+// *regen (may be null): what the frames of a splittable item regenerate -- their declared sizes, or all of `capacity` when the last zstd
+// frame declares none; *mostBlocks (may be null): the most blocks of one of the frames walked.
+ZB_HDN u32 item_walk(const u8* src, size_t size, u64 capacity, ItemFrame* out, u32 outMax, bool* split, u32 magicless = 0,
+                     u64* regen = nullptr, u32* mostBlocks = nullptr) {
+    u32 most = 0;
     u32 n = 0; size_t pos = 0; u64 declared = 0;
     bool sized = true, ok = true;      // sized: every zstd frame so far declares its content size
     while (pos < size) {
@@ -127,11 +131,14 @@ ZB_HDN u32 item_walk(const u8* src, size_t size, u64 capacity, ItemFrame* out, u
             f.srcSize = end; f.nBlocks = nb; f.checksum = fh.checksum; f.hasContentSize = fh.hasContentSize; f.contentSize = fh.contentSize;
             if (fh.hasContentSize) declared += fh.contentSize <= capacity ? fh.contentSize : capacity + 1;      // (no wrap)
             else sized = false;
+            most = nb > most ? nb : most;
         }
         if (out && n < outMax) out[n] = f;
         n++; pos += (size_t)f.srcSize;
     }
     *split = ok && pos == size && n >= 2 && declared <= capacity;
+    if (regen) *regen = sized ? declared : capacity;
+    if (mostBlocks) *mostBlocks = most;
     return n;
 }
 

@@ -1,6 +1,7 @@
-// zb_decode_list.cuh -- host side of the host-memory decompression calls: the decode list, which cuts items of several frames into their frames.
+// zb_decode_list.cuh -- the decode list, which cuts items of several frames into their frames: planned on the host for the host-memory
+// decompression calls (plan_decode_list), on the GPU for the device-memory call (split_device_*, kernels k_split_* in zb_capi.cu).
 //
-// An item item_walk lets split (zb_decode_fast.cuh) becomes one entry per frame -- a skippable frame too: it regenerates nothing, so
+// An item the split rule takes (split_entries) becomes one entry per frame -- a skippable frame too: it regenerates nothing, so
 // its capacity is 0 -- output at the item's output plus the declared sizes of the frames before it, capacity its own declared size (the
 // last entry: the rest of the item's).  Every other item is one entry.  The staged, segment and fused decoders then run over the entries
 // as over items, so every entry costs the staged decoder's per-item workspace (about 0.5 MB, per launch part of at most
@@ -18,6 +19,64 @@ namespace zb {
 
 constexpr u64 SPLIT_MIN_BYTES = 32768;      // bytes regenerated per entry, on average, by an item that is split (the staged workspace
                                             // of an entry is about 15 times that)
+
+// The split rule: the number of entries item src[0, size) of output capacity `cap` is cut into -- its frames -- or 0 when it is decoded
+// whole.  An item is split when item_walk lets it be and it regenerates at least SPLIT_MIN_BYTES per entry on average.
+// *mostBlocks: the most blocks of one of its frames.
+ZB_HDN u32 split_entries(const u8* src, size_t size, u64 cap, u32 magicless, u32* mostBlocks = nullptr) {
+    bool ok = false; u64 bytes = 0; u32 most = 0;
+    u32 const nf = item_walk(src, size, cap, nullptr, 0, &ok, magicless, &bytes, &most);
+    if (mostBlocks) *mostBlocks = most;
+    return ok && bytes / nf >= SPLIT_MIN_BYTES ? nf : 0;
+}
+
+// ---------------------------------------------------------------------------------------- the device call's list
+// zstdb200_decompress_device plans on the GPU: every item is counted (split_device_count), the counts are scanned into each item's first
+// entry, and the frames of every item taken are written to its entries (split_device_fill) -- plan_decode_list's entries in its order,
+// less those of the items kept whole.  The list holds at most `max` entries; an item whose entries would end beyond it is not taken.
+// The staged pipeline decodes the entries in parts (split_range), and each entry's result settles into its item (split_entry_stands):
+// the item's result is the sum of its entries', or the item is marked and the fused decoder decodes it again whole.
+
+// The entries of an item the device call splits: the split rule's, when every zstd frame of the item is one block (skippable frames
+// allowed; frames of several blocks stay with the segment loop).  0: the item is routed as without splitting.
+ZB_HDN u32 split_device_count(const u8* src, size_t size, u64 cap, u32 magicless) {
+    u32 most = 0;
+    u32 const nf = split_entries(src, size, cap, magicless, &most);
+    return most == 1 ? nf : 0;
+}
+
+// Whether item i is split: it has entries [first[i], first[i + 1]) and they fit the list of `max` entries (first null: none is).
+ZB_HD bool split_taken(const u64* first, u64 i, u64 max) { return first && first[i + 1] > first[i] && first[i + 1] <= max; }
+
+// The `count` entries of item i (input src[0, size), output at dstAt of capacity cap): its frames to frames[0 .. count), the output
+// offset of each to dst[0 .. count), i to item[0 .. count).
+ZB_HDN void split_device_fill(const u8* src, size_t size, u64 dstAt, u64 cap, u32 magicless, u32 i, u32 count, ItemFrame* frames, u64* dst,
+                              u32* item) {
+    bool ok = false;
+    item_walk(src, size, cap, frames, count, &ok, magicless);
+    u64 d = dstAt;
+    for (u32 q = 0; q < count; q++) {
+        dst[q] = d; item[q] = i;
+        if (!frames[q].skippable) d += frames[q].hasContentSize ? frames[q].contentSize : dstAt + cap - d;
+    }
+}
+
+// Entry j of the m listed: its input [src, srcEnd) and output [dst, dstEnd), offsets in the call's buffers (srcOff, dstOff: the items').
+// An item's last entry ends where the item does.
+struct SplitRange { u64 src, srcEnd, dst, dstEnd; };
+ZB_HD SplitRange split_range(const ItemFrame* frames, const u64* dst, const u32* item, u64 j, u64 m, const u64* srcOff, const u64* dstOff) {
+    u32 const i = item[j];
+    SplitRange r;
+    r.src = srcOff[i] + frames[j].srcOff; r.srcEnd = r.src + frames[j].srcSize;
+    r.dst = dst[j]; r.dstEnd = j + 1 < m && item[j + 1] == i ? dst[j + 1] : dstOff[i + 1];
+    return r;
+}
+
+// Whether an entry's result r stands for its frame: no error, and exactly the declared size (a skippable frame: nothing; a last frame
+// without a declared size: whatever fit).  When one does not, its item is decoded again whole.
+ZB_HD bool split_entry_stands(const ItemFrame& f, u64 r) {
+    return !isErr((size_t)r) && (f.skippable ? r == 0 : !f.hasContentSize || r == f.contentSize);
+}
 
 struct DecodeList {
     size_t m = 0;                        // entries
@@ -50,15 +109,12 @@ void plan_decode_list(DecodeList& L, size_t n, const u8* staged, const u64* srcO
         for (size_t i = 0; i < n; i++) {
             size_t const size = (size_t)(srcOff[i + 1] - srcOff[i]);
             u64 const cap = dstOff[i + 1] - dstOff[i];
-            bool ok = false;
-            u32 const nf = item_walk(staged + srcOff[i], size, cap, nullptr, 0, &ok, magicless);
-            if (!ok) continue;
+            u32 const nf = split_entries(staged + srcOff[i], size, cap, magicless);
+            if (!nf) continue;
             size_t const at = frames.size();
             frames.resize(at + nf);
+            bool ok = false;
             item_walk(staged + srcOff[i], size, cap, frames.data() + at, nf, &ok, magicless);
-            u64 bytes = 0;      // what the item's frames regenerate: their declared sizes, or all of the capacity when the last declares none
-            for (size_t k = at; k < at + nf; k++) if (!frames[k].skippable) bytes = frames[k].hasContentSize ? bytes + frames[k].contentSize : cap;
-            if (bytes / nf < SPLIT_MIN_BYTES) { frames.resize(at); continue; }
             L.split[i] = 1; count[i] = nf; m += nf - 1;
         }
         if (m == n) return;
