@@ -48,6 +48,10 @@ ZB_HDN u32 split_device_count(const u8* src, size_t size, u64 cap, u32 magicless
 // Whether item i is split: it has entries [first[i], first[i + 1]) and they fit the list of `max` entries (first null: none is).
 ZB_HD bool split_taken(const u64* first, u64 i, u64 max) { return first && first[i + 1] > first[i] && first[i + 1] <= max; }
 
+// The output offset of the entry after frame f's, which starts at d in an item whose output ends at `end`: a skippable frame takes
+// nothing, a frame its declared size, a frame without one the rest of the item's capacity.
+ZB_HD u64 split_next_dst(const ItemFrame& f, u64 d, u64 end) { return f.skippable ? d : f.hasContentSize ? d + f.contentSize : end; }
+
 // The `count` entries of item i (input src[0, size), output at dstAt of capacity cap): its frames to frames[0 .. count), the output
 // offset of each to dst[0 .. count), i to item[0 .. count).
 ZB_HDN void split_device_fill(const u8* src, size_t size, u64 dstAt, u64 cap, u32 magicless, u32 i, u32 count, ItemFrame* frames, u64* dst,
@@ -57,7 +61,7 @@ ZB_HDN void split_device_fill(const u8* src, size_t size, u64 dstAt, u64 cap, u3
     u64 d = dstAt;
     for (u32 q = 0; q < count; q++) {
         dst[q] = d; item[q] = i;
-        if (!frames[q].skippable) d += frames[q].hasContentSize ? frames[q].contentSize : dstAt + cap - d;
+        d = split_next_dst(frames[q], d, dstAt + cap);
     }
 }
 
@@ -129,7 +133,7 @@ void plan_decode_list(DecodeList& L, size_t n, const u8* staged, const u64* srcO
                 ItemFrame const& f = frames[k++];
                 L.frame[L.src.size()] = f;
                 L.src.push_back(srcOff[i] + f.srcOff); L.dst.push_back(d);
-                if (!f.skippable) d += f.hasContentSize ? f.contentSize : dstOff[i + 1] - d;
+                d = split_next_dst(f, d, dstOff[i + 1]);
             }
         }
         L.src.push_back(srcOff[n]); L.dst.push_back(dstOff[n]); L.first[n] = m;
