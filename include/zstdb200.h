@@ -310,6 +310,25 @@ ZSTDB200_API size_t zstdb200_compress_device(zstdb200_ctx* ctx, int level, size_
                                              void* d_slots, size_t slotStride, uint64_t* d_frameSizes, void* stream);
 ZSTDB200_API size_t zstdb200_compact_device(zstdb200_ctx* ctx, size_t n, const void* d_slots, size_t slotStride, const uint64_t* d_frameSizes,
                                             void* d_out, uint64_t* d_outOffsets, void* stream);
+/* compress_items_device compresses n items, item i = d_src[d_srcOffsets[i] .. d_srcOffsets[i+1]), each into the stream ZSTD_compress2
+ * writes for it with ZSTDB200_c_multiFrame: one frame per chunkSize piece, each frame byte-identical to the reference's one-shot frame of
+ * that piece at `level` and the context's frame options (checksum, content_size, magicless, explicit c_* parameters); an empty item is
+ * the one empty frame.  The streams are packed in item order into d_dst: item i at [d_dstOffsets[i], d_dstOffsets[i+1]) (n+1 entries),
+ * d_results[i] its size or the first error code among its frames.  The items are cut, compressed and packed on the GPU; nothing in the
+ * call waits on the host.
+ *   - chunkSize 0 or above 131072: parameter_outOfBound; a level without a GPU parser: parameter_unsupported (both returned, nothing queued).
+ *   - dstCapacity must reach the sum, over every item's chunks, of ZSTD_compressBound(chunk), as for zstdb200_compress_chunks; when it
+ *     does not, every item reports dstSize_tooSmall, every offset is 0 and nothing is compressed.
+ *   - a frame the GPU does not serve (an optimal level on a chunk over 64 KB, levels 11-12 on a chunk of at most 16 KB) reports
+ *     parameter_unsupported, and so does its item; the other items are unaffected.
+ * The chunks are compressed in parts of P = min(16384, n + dstCapacity / chunkSize) by a CUDA graph the context keeps (built on the
+ * first call and again when P, the level, chunkSize or a compression option changes); its workspace -- about 0.65 MB per part slot at
+ * chunkSize 131072, the sequence records and the frame slots, and 40 bytes per item -- is kept too.  When the workspace or the graph
+ * cannot be had the call returns memory_allocation and leaves neither the CUDA error state nor zstdb200_last_error() a trace.  The call
+ * uses the context's work set 0 and must not overlap another call on it. */
+ZSTDB200_API size_t zstdb200_compress_items_device(zstdb200_ctx* ctx, int level, size_t chunkSize, size_t n, const void* d_src,
+                                                   const uint64_t* d_srcOffsets, void* d_dst, size_t dstCapacity, uint64_t* d_dstOffsets,
+                                                   uint64_t* d_results, void* stream);
 /* decompress_device regenerates item i into d_dst + d_dstOffsets[i] (capacity d_dstOffsets[i+1] - d_dstOffsets[i]) and writes its size or
  * error code to d_results[i].  With dec_pipeline on (the default) the items are routed on the GPU: single-block frames with a content size
  * go to the staged decoder; items of several frames that are all one block are cut into their frames on the GPU, by the rule the

@@ -131,6 +131,7 @@ def lib() -> C.CDLL:
     sig("zstdb200_sequenceProducer", sz, vp, vp, sz, vp, sz, vp, sz, i, sz)
     sig("zstdb200_compress_device", sz, vp, i, sz, vp, vp, vp, sz, vp, vp)
     sig("zstdb200_compact_device", sz, vp, sz, vp, sz, vp, vp, vp, vp)
+    sig("zstdb200_compress_items_device", sz, vp, i, sz, sz, vp, vp, vp, sz, vp, vp, vp)
     sig("zstdb200_decompress_device", sz, vp, sz, vp, vp, vp, vp, vp, vp)
     sig("zstdb200_sync", sz, vp, vp)
     _lib = L
