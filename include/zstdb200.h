@@ -345,6 +345,33 @@ ZSTDB200_API size_t zstdb200_compress_items_device(zstdb200_ctx* ctx, int level,
  * do not count device calls. */
 ZSTDB200_API size_t zstdb200_decompress_device(zstdb200_ctx* ctx, size_t n, const void* d_src, const uint64_t* d_srcOffsets,
                                                void* d_dst, const uint64_t* d_dstOffsets, uint64_t* d_results, void* stream);
+/* decompress_bound_device finds on the GPU the room every item needs, from its frames alone.  d_bounds[i] (d_bounds may be NULL) is
+ * ZSTD_decompressBound of item i = d_src[d_srcOffsets[i] .. d_srcOffsets[i+1]): the sum over its frames of the declared content size, or
+ * the frame's blocks times its largest block size for a frame that declares none; skippable frames count 0; ZSTD_CONTENTSIZE_ERROR for
+ * an item that is not a whole number of frames whose headers are valid.  On a magicless context the frames are ZSTD_f_zstd1_magicless
+ * frames, and there are no skippable ones.  Item i's room is its bound, or 0 when the bound is ZSTD_CONTENTSIZE_ERROR; d_dstOffsets
+ * (n+1 entries) is the exclusive scan of the rooms, the sum saturating at 2^64-1.  Nothing in the call waits on the host.
+ *   - n above 2^31-1: srcSize_wrong (returned, nothing queued); n == 0 writes d_dstOffsets[0] = 0.
+ *   - with d_bounds NULL the bounds go to a workspace the context keeps (8 bytes per item); when it cannot be had the call returns
+ *     memory_allocation and leaves neither the CUDA error state nor zstdb200_last_error() a trace.
+ * The call uses the context's work set 0 and must not overlap another call on it. */
+ZSTDB200_API size_t zstdb200_decompress_bound_device(zstdb200_ctx* ctx, size_t n, const void* d_src, const uint64_t* d_srcOffsets,
+                                                     uint64_t* d_dstOffsets, uint64_t* d_bounds, void* stream);
+/* decompress_items_device regenerates items whose sizes only their frames know.  It writes d_dstOffsets as decompress_bound_device does,
+ * then checks d_dstOffsets[n] <= dstCapacity on the GPU.
+ *   - When the rooms fit, it decodes as zstdb200_decompress_device with those offsets: item i into d_dst + d_dstOffsets[i], d_results[i]
+ *     its size or error code, each the same as zstdb200_decompress_device gives for these rooms.  The output is packed exactly when every
+ *     frame declares its content size (the frames this library writes, and the reference's one-shot frames); otherwise the rooms are
+ *     bounds, and d_results[i] says how much of item i's room was regenerated.
+ *   - When they do not fit, every item reports dstSize_tooSmall and nothing is written to d_dst.  d_dstOffsets still holds the plan: a
+ *     caller can read d_dstOffsets[n], allocate that much and call again.
+ *   - n above 2^31-1: srcSize_wrong (returned, nothing queued); n == 0 writes d_dstOffsets[0] = 0.
+ * With dec_pipeline 0 the plan is the same and the fused kernel decodes.  Nothing in the call waits on the host.  Besides
+ * zstdb200_decompress_device's workspaces, the call keeps 24 bytes per item; when that cannot be had it returns memory_allocation and
+ * leaves neither the CUDA error state nor zstdb200_last_error() a trace.  The call uses the context's work set 0 and must not overlap
+ * another call on it. */
+ZSTDB200_API size_t zstdb200_decompress_items_device(zstdb200_ctx* ctx, size_t n, const void* d_src, const uint64_t* d_srcOffsets, void* d_dst,
+                                                     size_t dstCapacity, uint64_t* d_dstOffsets, uint64_t* d_results, void* stream);
 ZSTDB200_API size_t zstdb200_sync(zstdb200_ctx* ctx, void* stream);
 
 #ifdef __cplusplus

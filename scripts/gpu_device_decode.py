@@ -11,9 +11,11 @@ against the fused kernel alone (dec_pipeline 0).  Warm, best of 3, outputs compa
 The one-frame items go to the staged decoder, the two-block files to the fused kernel (many short items), the long frames to the
 segment loop; the items of several one-block frames are cut into their frames for the staged decoder.  Prints one JSON line with the
 card's name and power limit.
-    python scripts/gpu_device_decode.py [--mb 1024] [--lib path/to/libzstdb200.so] [--many-only]
+    python scripts/gpu_device_decode.py [--mb 1024] [--lib path/to/libzstdb200.so] [--many-only] [--items]
 --lib measures another build of the library (an earlier commit); --many-only times only the many-item workloads (an earlier build
-decodes the long items with one warp each, minutes per GiB).
+decodes the long items with one warp each, minutes per GiB).  --items also times, on every device workload, alternating with the device
+call on host-planned offsets: zstdb200_decompress_items_device, which finds the rooms on the GPU ("items"), and
+zstdb200_decompress_bound_device alone ("plan_ms"); plan_share is plan_ms over the items call's time.
 """
 from __future__ import annotations
 
@@ -43,6 +45,7 @@ def main():
     ap.add_argument("--mb", type=int, default=1024)
     ap.add_argument("--lib", default="")
     ap.add_argument("--many-only", action="store_true")
+    ap.add_argument("--items", action="store_true")
     args = ap.parse_args()
     if args.lib:
         os.environ["ZSTDB200_LIBRARY"] = args.lib
@@ -56,25 +59,45 @@ def main():
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
 
     def device_rate(ctx, items, contents):
+        n = len(items)
         so = np.concatenate([[0], np.cumsum([len(x) for x in items])]).astype(np.int64)
         do = np.concatenate([[0], np.cumsum([len(x) for x in contents])]).astype(np.int64)
         d_src = torch.from_numpy(np.frombuffer(b"".join(items), dtype=np.uint8).copy()).to(dev)
         d_so, d_do = torch.from_numpy(so).to(dev), torch.from_numpy(do).to(dev)
         d_dst = torch.zeros(int(do[-1]), dtype=torch.uint8, device=dev)
-        d_res = torch.zeros(len(items), dtype=torch.int64, device=dev)
+        d_res = torch.zeros(n, dtype=torch.int64, device=dev)
+        d_plan = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        d_bounds = torch.zeros(n, dtype=torch.int64, device=dev)
         s = torch.cuda.Stream()
-        best = None
+        calls = {"device": lambda: L.zstdb200_decompress_device(ctx.handle, n, d_src.data_ptr(), d_so.data_ptr(), d_dst.data_ptr(),
+                                                                d_do.data_ptr(), d_res.data_ptr(), s.cuda_stream)}
+        if args.items:
+            calls["items"] = lambda: L.zstdb200_decompress_items_device(ctx.handle, n, d_src.data_ptr(), d_so.data_ptr(), d_dst.data_ptr(),
+                                                                        int(do[-1]), d_plan.data_ptr(), d_res.data_ptr(), s.cuda_stream)
+            calls["plan"] = lambda: L.zstdb200_decompress_bound_device(ctx.handle, n, d_src.data_ptr(), d_so.data_ptr(), d_plan.data_ptr(),
+                                                                       d_bounds.data_ptr(), s.cuda_stream)
+        best, ok = {}, {}
         for rep in range(4):
-            d_dst.zero_(); torch.cuda.synchronize()
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record(s)
-            assert L.zstdb200_decompress_device(ctx.handle, len(items), d_src.data_ptr(), d_so.data_ptr(), d_dst.data_ptr(), d_do.data_ptr(),
-                                                d_res.data_ptr(), s.cuda_stream) == 0
-            b.record(s); s.synchronize()
-            if rep:
-                best = min(best or 1e9, a.elapsed_time(b))
-        ok = d_res.cpu().tolist() == [len(x) for x in contents] and bytes(d_dst.cpu().numpy()) == b"".join(contents)
-        return {"GBps": round(int(do[-1]) / best / 1e6, 3), "ms": round(best, 3), "ok": ok}
+            for name, call in calls.items():      # alternating, so that drift on the card touches every call alike
+                d_dst.zero_(); d_plan.zero_(); torch.cuda.synchronize()
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record(s)
+                assert call() == 0
+                b.record(s); s.synchronize()
+                if rep:
+                    best[name] = min(best.get(name, 1e9), a.elapsed_time(b))
+                if name == "plan":
+                    ok[name] = d_plan.cpu().tolist() == do.tolist()
+                else:
+                    ok[name] = d_res.cpu().tolist() == [len(x) for x in contents] and bytes(d_dst.cpu().numpy()) == b"".join(contents)
+                    ok[name] = ok[name] and (name == "device" or d_plan.cpu().tolist() == do.tolist())
+        rate = lambda k: {"GBps": round(int(do[-1]) / best[k] / 1e6, 3), "ms": round(best[k], 3), "ok": ok[k]}
+        out = rate("device")
+        if args.items:
+            out["items"] = rate("items")
+            out["plan_ms"], out["plan_ok"] = round(best["plan"], 4), ok["plan"]
+            out["plan_share"] = round(best["plan"] / best["items"], 5)
+        return out
 
     def frames_rate(ctx, frame, content):
         out = C.create_string_buffer(len(content))
