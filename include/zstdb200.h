@@ -372,6 +372,36 @@ ZSTDB200_API size_t zstdb200_decompress_bound_device(zstdb200_ctx* ctx, size_t n
  * another call on it. */
 ZSTDB200_API size_t zstdb200_decompress_items_device(zstdb200_ctx* ctx, size_t n, const void* d_src, const uint64_t* d_srcOffsets, void* d_dst,
                                                      size_t dstCapacity, uint64_t* d_dstOffsets, uint64_t* d_results, void* stream);
+/* decompress_ranges_device regenerates byte ranges of items, decoding only the frames that hold them.  Item i is
+ * d_src[d_srcOffsets[i] .. d_srcOffsets[i+1]) (n+1 offsets).  Request r (m of them) asks for the regenerated bytes
+ * [d_rangeBegins[r], d_rangeBegins[r] + len_r) of item d_rangeItems[r], len_r = d_dstOffsets[r+1] - d_dstOffsets[r] (m+1 offsets); they
+ * go to d_dst + d_dstOffsets[r], and d_results[r] receives the number of bytes written or an error code.
+ *   - Only the frames that regenerate at least one byte of a range are decoded.  The frames before it are walked (their headers and block
+ *     headers), not decoded; the frames after it are not read.  A damaged frame outside a range does not affect that request.
+ *   - Every frame covered is decoded whole and its checksum, if any, verified.  It must regenerate exactly its declared size, else the
+ *     result is corruption_detected; its decode error is the one zstdb200_decompress_device gives for that frame alone in a room of its declared size.
+ *   - When the item's content ends before the range does, the result is the bytes up to its end (as pread); a range starting at or past
+ *     the end gives 0.  Bytes of the request's output beyond a short read are not written.
+ *   - Every zstd frame the walk passes before the range's end must declare its content size, else the request gives
+ *     parameter_unsupported.  Skippable frames and empty frames are walked and count 0.
+ *   - A frame the range covers only in part must declare at most 131072 bytes (every frame compress_items_device, compress_chunks and the
+ *     reference's one-shot path write does), else parameter_unsupported.  Frames of any size covered wholly decode straight into d_dst.
+ *   - An item that cannot be walked as far as the range reaches gives the error ZSTD_findFrameCompressedSize gives for the first frame
+ *     it cannot pass.  Where several failures apply, the first in item order wins.
+ *   - d_rangeItems[r] >= n gives parameter_outOfBound; len_r == 0 gives 0 and reads nothing.
+ *   - A failed request's output is unspecified, but nothing is ever written outside [d_dstOffsets[r], d_dstOffsets[r+1]).
+ *   - m or n above 2^31-1: srcSize_wrong (returned, nothing queued); m == 0 queues nothing.
+ * On a magicless context the items are ZSTD_f_zstd1_magicless frames, with no skippable frames.  With dec_pipeline 0 the plan is the
+ * same and the fused kernel decodes.  Nothing in the call waits on the host.  The covered frames are decoded in parts of
+ * P = min(16384, max(512, m)) frames, at most P / 2 of them covered in part, by a CUDA graph the context keeps (built on the first call
+ * and again when P or a decoding option changes).  Its workspace does not grow with the ranges' lengths or frame counts: 64 bytes per
+ * request, P / 2 scratch slots of 128 KB (32 MB at P = 512, 1 GB at P = 16384), 89 bytes per part slot, and the decoders' workspace for
+ * P frames, which zstdb200_decompress_device's decode list shares.  When any of it cannot be had the call returns memory_allocation and
+ * leaves neither the CUDA error state nor zstdb200_last_error() a trace.  The call uses the context's work set 0 and must not overlap
+ * another call on it. */
+ZSTDB200_API size_t zstdb200_decompress_ranges_device(zstdb200_ctx* ctx, size_t n, const void* d_src, const uint64_t* d_srcOffsets,
+                                                      size_t m, const uint64_t* d_rangeItems, const uint64_t* d_rangeBegins,
+                                                      void* d_dst, const uint64_t* d_dstOffsets, uint64_t* d_results, void* stream);
 ZSTDB200_API size_t zstdb200_sync(zstdb200_ctx* ctx, void* stream);
 
 #ifdef __cplusplus

@@ -135,6 +135,7 @@ def lib() -> C.CDLL:
     sig("zstdb200_decompress_device", sz, vp, sz, vp, vp, vp, vp, vp, vp)
     sig("zstdb200_decompress_bound_device", sz, vp, sz, vp, vp, vp, vp, vp)
     sig("zstdb200_decompress_items_device", sz, vp, sz, vp, vp, vp, sz, vp, vp, vp)
+    sig("zstdb200_decompress_ranges_device", sz, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp, vp)
     sig("zstdb200_sync", sz, vp, vp)
     _lib = L
     return L

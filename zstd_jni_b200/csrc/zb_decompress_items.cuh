@@ -13,42 +13,51 @@ namespace zb {
 
 constexpr u64 CONTENTSIZE_UNKNOWN = ~0ull, CONTENTSIZE_ERROR = ~0ull - 1;      // ZSTD_CONTENTSIZE_UNKNOWN / ZSTD_CONTENTSIZE_ERROR
 
-// ZSTD_decompressBound of item src[0, size) (N/decompress/zstd_decompress.c:734-836): the sum over its frames of the declared content
-// size, or, for a frame that declares none, its blocks times its largest block; skippable frames count nothing; CONTENTSIZE_ERROR when the
-// item is not a whole number of frames whose headers read.  Frames of any size are walked (frame_walk stops at 4 GiB).  A magicless item
-// has no skippable frames (the reference's ZSTD_f_zstd1_magicless walk).  As in the reference, a declared size of CONTENTSIZE_UNKNOWN
-// counts as none, one of CONTENTSIZE_ERROR is an error, and the sum wraps.
+// ZSTD_findFrameSizeInfo (N/decompress/zstd_decompress.c:734-799) of the frame that starts src[0, size): its header to *fh, its blocks to
+// *blocks (0 for a skippable frame); returns its compressed size, or the error ZSTD_findFrameCompressedSize gives for it.  Frames of any
+// size are walked.  In the magicless format there are no skippable frames (the reference's ZSTD_f_zstd1_magicless walk).
+ZB_HDN size_t frame_size_info(const u8* src, size_t size, u32 magicless, FrameHeader* fh, u64* blocks) {
+    *blocks = 0;
+    {   size_t const r = read_frame_header(fh, src, size, magicless);
+        if (r != 0) return isErr(r) ? r : ERR(E_srcSize_wrong); }      // an error, or a header cut short
+    if (fh->skippable) {      // readSkippableFrameSize: a length whose frame size wraps 32 bits is refused
+        if (fh->skipLen > 0xFFFFFFF7u) return ERR(E_frameParameter_unsupported);
+        if ((u64)fh->skipLen + 8 > size) return ERR(E_srcSize_wrong);
+        return 8 + (size_t)fh->skipLen;
+    }
+    size_t p = fh->headerSize;
+    for (;;) {      // ZSTD_getcBlockSize, then the block inside the input
+        if (size - p < 3) return ERR(E_srcSize_wrong);
+        u32 const bh = load24(src + p), type = (bh >> 1) & 3;
+        size_t const cSize = type == 1 ? 1 : bh >> 3;
+        if (type == 3) return ERR(E_corruption_detected);
+        if (cSize > size - p - 3) return ERR(E_srcSize_wrong);
+        p += 3 + cSize; ++*blocks;
+        if (bh & 1) break;
+    }
+    if (fh->checksum) {
+        if (size - p < 4) return ERR(E_srcSize_wrong);
+        p += 4;
+    }
+    return p;
+}
+
+// ZSTD_decompressBound of item src[0, size) (N/decompress/zstd_decompress.c:734-836): the sum over its frames (frame_size_info) of the
+// declared content size, or, for a frame that declares none, its blocks times its largest block; skippable frames count nothing;
+// CONTENTSIZE_ERROR when the item is not a whole number of frames whose headers read.  As in the reference, a declared size of
+// CONTENTSIZE_UNKNOWN counts as none, one of CONTENTSIZE_ERROR is an error, and the sum wraps.
 ZB_HDN u64 ditem_bound(const u8* src, size_t size, u32 magicless) {
     u64 bound = 0;
     size_t pos = 0;
     while (pos < size) {
-        size_t const rest = size - pos;
-        const u8* const f = src + pos;
-        FrameHeader fh;
-        if (read_frame_header(&fh, f, rest, magicless) != 0) return CONTENTSIZE_ERROR;      // an error, or a header cut short
-        if (fh.skippable) {      // (readSkippableFrameSize: a length whose frame size wraps 32 bits is refused)
-            if (fh.skipLen > 0xFFFFFFF7u || (u64)fh.skipLen + 8 > rest) return CONTENTSIZE_ERROR;
-            pos += 8 + (size_t)fh.skipLen;
-            continue;
-        }
-        size_t p = fh.headerSize;
-        u64 blocks = 0;
-        for (;;) {
-            if (rest - p < 3) return CONTENTSIZE_ERROR;
-            u32 const bh = load24(f + p), type = (bh >> 1) & 3;
-            size_t const cSize = type == 1 ? 1 : bh >> 3;
-            if (type == 3 || cSize > rest - p - 3) return CONTENTSIZE_ERROR;
-            p += 3 + cSize; blocks++;
-            if (bh & 1) break;
-        }
-        if (fh.checksum) {
-            if (rest - p < 4) return CONTENTSIZE_ERROR;
-            p += 4;
-        }
+        FrameHeader fh; u64 blocks;
+        size_t const fs = frame_size_info(src + pos, size - pos, magicless, &fh, &blocks);
+        if (isErr(fs)) return CONTENTSIZE_ERROR;
+        pos += fs;
+        if (fh.skippable) continue;
         u64 const declared = fh.hasContentSize ? fh.contentSize : CONTENTSIZE_UNKNOWN;
         if (declared == CONTENTSIZE_ERROR) return CONTENTSIZE_ERROR;
         bound += declared != CONTENTSIZE_UNKNOWN ? declared : blocks * fh.blockSizeMax;
-        pos += p;
     }
     return bound;
 }
