@@ -180,7 +180,9 @@ ZSTDB200_API int zstdb200_device_count(void);
  *   "entropy_overlap" (0|1, default 1: the entropy stage is launched as a programmatic dependent of the parse and
  *   takes frames in the order their parse finishes, filling the SMs the parse's tail leaves idle),
  *   "kernel_fifo" (0|1, default 1: the kernel sections of host-memory operations queued on different work sets run
- *   one after the other in submission order -- copies still overlap them; two batches in the kernels at once only slow each other down).
+ *   one after the other in submission order -- copies still overlap them; two batches in the kernels at once only slow each other down),
+ *   "seek_table" (0|1, default 0: compress_items_device writes the seekable format's seek table after every item, and
+ *   decompress_ranges_device locates ranges through such tables; see those calls; no environment variable).
  * zstdb200_create reads these ten from the environment (a value the option rejects is ignored): ZSTDB200_ENC_WARPS_PER_SM,
  * ZSTDB200_DEC_WARPS_PER_SM, ZSTDB200_PARSE_LANES, ZSTDB200_PARSE_BLOCKS_PER_SM, ZSTDB200_LAZY_BLOCKS_PER_SM, ZSTDB200_PARSE_EST_BYTES,
  * ZSTDB200_L2_FETCH (l2_fetch_granularity), ZSTDB200_HOST_SLICES, ZSTDB200_ENTROPY_OVERLAP and ZSTDB200_KERNEL_FIFO. */
@@ -325,7 +327,16 @@ ZSTDB200_API size_t zstdb200_compact_device(zstdb200_ctx* ctx, size_t n, const v
  * first call and again when P, the level, chunkSize or a compression option changes); its workspace -- about 0.65 MB per part slot at
  * chunkSize 131072, the sequence records and the frame slots, and 40 bytes per item -- is kept too.  When the workspace or the graph
  * cannot be had the call returns memory_allocation and leaves neither the CUDA error state nor zstdb200_last_error() a trace.  The call
- * uses the context's work set 0 and must not overlap another call on it. */
+ * uses the context's work set 0 and must not overlap another call on it.
+ * With option "seek_table" 1 each item is followed by its seek table (zstd's seekable format): a skippable frame of magic 0x184D2A5E
+ * holding one entry per frame -- its compressed size, its regenerated size, and when the "checksum" option is on the frame's content
+ * checksum (the descriptor's checksum flag is then set) -- then the frame count, the descriptor and 0x8F92EAB1.  The frames are the same
+ * bytes as with the option off; item i is the option-off stream followed by its table, and d_results[i] and d_dstOffsets count the table.
+ *   - dstCapacity must also reach 8 + E * k_i + 9 more bytes per item of k_i chunks (E = 12 with checksums, else 8); one byte short
+ *     gives dstSize_tooSmall for every item as above.
+ *   - an item of more than 0x8000000 chunks reports frameIndex_tooLarge; the other items are unaffected.  An item that fails has no table.
+ *   - together with "magicless" the call returns parameter_unsupported and queues nothing.
+ * The table's bookkeeping adds 8 bytes of kept workspace per chunk the capacity could hold. */
 ZSTDB200_API size_t zstdb200_compress_items_device(zstdb200_ctx* ctx, int level, size_t chunkSize, size_t n, const void* d_src,
                                                    const uint64_t* d_srcOffsets, void* d_dst, size_t dstCapacity, uint64_t* d_dstOffsets,
                                                    uint64_t* d_results, void* stream);
@@ -398,7 +409,21 @@ ZSTDB200_API size_t zstdb200_decompress_items_device(zstdb200_ctx* ctx, size_t n
  * request, P / 2 scratch slots of 128 KB (32 MB at P = 512, 1 GB at P = 16384), 89 bytes per part slot, and the decoders' workspace for
  * P frames, which zstdb200_decompress_device's decode list shares.  When any of it cannot be had the call returns memory_allocation and
  * leaves neither the CUDA error state nor zstdb200_last_error() a trace.  The call uses the context's work set 0 and must not overlap
- * another call on it. */
+ * another call on it.
+ * With option "seek_table" 1 a request whose item ends with a valid seek table is located through it, without walking the frames before
+ * the range.  Valid: the item is at least 17 bytes and ends with 0x8F92EAB1, the descriptor's reserved bits (6-2) are 0, the frame count
+ * k is at most 0x8000000, the table (8 + E k + 9 bytes) fits the item and starts with 0x184D2A5E and E k + 9, and the entries'
+ * compressed sizes sum to exactly the bytes before it.  Any other item is walked as with the option off, with the same results.
+ * Through a table:
+ *   - entries of regenerated size 0 are passed; an entry that holds a byte of the range is decoded, and frames need not declare their
+ *     content size.  An entry covered in part must regenerate at most 131072 bytes, else parameter_unsupported.
+ *   - each decoded entry's frame must be walkable (else ZSTD_findFrameCompressedSize's error), not skippable, of the entry's compressed
+ *     size and, if it declares a content size, of the entry's regenerated size (else corruption_detected); it must regenerate exactly
+ *     that size, with the error rule above; and with the table's checksum flag its bytes must hash to the entry's checksum (the low 32
+ *     bits of XXH64), else checksum_wrong.  The first failure in item order still wins.
+ *   - the content ends at the sum of the entries' regenerated sizes; short reads and ranges past the end are as above.
+ *   - together with "magicless" the call returns parameter_unsupported and queues nothing.
+ * The workspace is the same; the graph is built again when the option changes. */
 ZSTDB200_API size_t zstdb200_decompress_ranges_device(zstdb200_ctx* ctx, size_t n, const void* d_src, const uint64_t* d_srcOffsets,
                                                       size_t m, const uint64_t* d_rangeItems, const uint64_t* d_rangeBegins,
                                                       void* d_dst, const uint64_t* d_dstOffsets, uint64_t* d_results, void* stream);

@@ -9,6 +9,8 @@ For each: the new call (items in, packed multi-frame streams out, the chunks pla
 zstdb200_compact_device on the same 128 KB chunks, their offsets planned on the host beforehand (not timed).  Both write the same
 packed stream, which is compared byte for byte.  Times are CUDA events around each call on one stream, best of `reps` warm runs.
 Prints the card's name and power limit, read in the same run, and one JSON line per workload.
+With --seek-table the call is also timed with option seek_table on (tables_ms, alternating with the other two), and its output checked
+to be the option-off streams each followed by its table.
 """
 from __future__ import annotations
 
@@ -39,6 +41,7 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--levels", default="1,3")
+    ap.add_argument("--seek-table", action="store_true")
     args = ap.parse_args()
     import torch
     from zstd_jni_b200 import _native, corpus
@@ -52,7 +55,8 @@ def main():
     mixed = [int(x) for x in rng.integers(0, 300 << 10, size=20_000)]
     workloads = [("8192 x 128 KB", [CHUNK] * 8192), ("64 x 16 MB", [16 << 20] * 64), ("20000 x 0-300 KB", mixed)]
     lines = []
-    with ZstdBatchContext(0) as ctx:
+    with ZstdBatchContext(0) as ctx, ZstdBatchContext(0) as tctx:
+        tctx.setOption("seek_table", 1)
         s = torch.cuda.Stream()
         for name, sizes in workloads:
             total = sum(sizes)
@@ -71,6 +75,11 @@ def main():
             slots = torch.empty(m * stride, dtype=torch.uint8, device=dev)
             fsz = torch.zeros(m, dtype=torch.int64, device=dev)
             coff = torch.zeros(m + 1, dtype=torch.int64, device=dev)
+            ks = [max(1, -(-n // CHUNK)) for n in sizes]
+            tcap = cap + sum(17 + 8 * k for k in ks)
+            out_tab = torch.zeros(tcap if args.seek_table else 1, dtype=torch.uint8, device=dev)
+            dot = torch.zeros(len(sizes) + 1, dtype=torch.int64, device=dev)
+            rest = torch.zeros(len(sizes), dtype=torch.int64, device=dev)
             for level in [int(x) for x in args.levels.split(",")]:
                 def new():
                     assert L.zstdb200_compress_items_device(ctx.handle, level, CHUNK, len(sizes), src.data_ptr(), d_so.data_ptr(), out_new.data_ptr(),
@@ -82,9 +91,14 @@ def main():
                     assert L.zstdb200_compact_device(ctx.handle, m, slots.data_ptr(), stride, fsz.data_ptr(), out_old.data_ptr(), coff.data_ptr(),
                                                      s.cuda_stream) == 0
 
-                times = {"new": [], "pair": []}
+                def tables():
+                    assert L.zstdb200_compress_items_device(tctx.handle, level, CHUNK, len(sizes), src.data_ptr(), d_so.data_ptr(), out_tab.data_ptr(),
+                                                            tcap, dot.data_ptr(), rest.data_ptr(), s.cuda_stream) == 0
+
+                times = {"new": [], "pair": [], "tables": []}
+                calls = (("new", new), ("pair", old)) + ((("tables", tables),) if args.seek_table else ())
                 for rep in range(args.reps + 1):                  # the first round warms up (and builds the graph)
-                    for key, f in (("new", new), ("pair", old)):
+                    for key, f in calls:
                         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                         a.record(s)
                         f()
@@ -99,9 +113,17 @@ def main():
                         "new_ms": min(times["new"]), "pair_ms": min(times["pair"]), "new_GBps": total / min(times["new"]) / 1e6,
                         "pair_GBps": total / min(times["pair"]) / 1e6, "new_all_ms": times["new"], "pair_all_ms": times["pair"],
                         "same_output": same, "no_errors": ok, "ratio": total / max(n_new, 1)}
+                if args.seek_table:      # every item: the option-off stream, then 8 + 8 k + 9 bytes of table
+                    a, b = do.cpu().numpy(), dot.cpu().numpy()
+                    tables_ok = bool((rest >= 0).all().item()) and all(int(b[i + 1] - b[i]) == int(a[i + 1] - a[i]) + 17 + 8 * ks[i] for i in range(len(sizes)))
+                    step = max(1, len(sizes) // 64)
+                    tables_ok = tables_ok and all(torch.equal(out_tab[int(b[i]):int(b[i]) + int(a[i + 1] - a[i])], out_new[int(a[i]):int(a[i + 1])])
+                                                  for i in range(0, len(sizes), step))
+                    line.update({"tables_ms": min(times["tables"]), "tables_all_ms": times["tables"], "tables_ok": tables_ok})
+                    line["no_errors"] = ok and tables_ok
                 print(json.dumps(line), flush=True)
                 lines.append(line)
-            del src, slots, out_new, out_old
+            del src, slots, out_new, out_old, out_tab
             torch.cuda.empty_cache()
     if args.out:
         Path(args.out).mkdir(parents=True, exist_ok=True)

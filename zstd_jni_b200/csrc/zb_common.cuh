@@ -35,7 +35,7 @@ enum : int {
     E_corruption_detected = 20, E_checksum_wrong = 22, E_literals_headerWrong = 24, E_dictionary_corrupted = 30, E_dictionary_wrong = 32,
     E_parameter_unsupported = 40, E_parameter_outOfBound = 42, E_tableLog_tooLarge = 44, E_maxSymbolValue_tooLarge = 46,
     E_maxSymbolValue_tooSmall = 48, E_stage_wrong = 60, E_init_missing = 62, E_memory_allocation = 64, E_workSpace_tooSmall = 66,
-    E_dstSize_tooSmall = 70, E_srcSize_wrong = 72, E_dstBuffer_null = 74, E_sequenceProducer_failed = 106, E_externalSequences_invalid = 107,
+    E_dstSize_tooSmall = 70, E_srcSize_wrong = 72, E_dstBuffer_null = 74, E_frameIndex_tooLarge = 100, E_sequenceProducer_failed = 106, E_externalSequences_invalid = 107,
     E_maxCode = 120
 };
 ZB_HD size_t ERR(int code) { return (size_t)0 - (size_t)code; }
